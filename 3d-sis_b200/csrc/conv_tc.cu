@@ -42,6 +42,8 @@ struct TcArgs {
     __half *out16;                      // optional fp16 twin of the output (same geometry as `out`); `out` may be null
     const float *bias_mid;              // N2 > 0: bias of the 3x3x3 conv (added before the inner ReLU), or null
     int n_tiles;                        // bricks of this launch (the grid may be padded to a multiple of the cluster size)
+    __half *out_split;                  // X3 = 2, KS = 1: optional split-pair output ([32 hi | 32 lo] halves per voxel and
+                                        // 32-channel slice, row stride 2 cout); `out` may then be null
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -214,7 +216,8 @@ struct TcStages { static constexpr int value = BN >= 128 ? 4 : 3; };
 // stages (96 KB), BN = 64 two (88 KB), BN = 128 three (204 KB)
 // X3 = 2 (fp16 split, 128-byte fp32 source rows): a stage = the slab (fp32 as it lands, split IN PLACE into fp16 hi / lo tiles of
 // half the size each) + fp16 hi/lo weight tiles.  3x3x3: BN = 32: three stages of 32 KB, BN = 64: four of 44 KB, BN = 128:
-// three of 68 KB; 1x1 / 2x2x2 / GEMM: four.
+// three of 68 KB; 1x1 / 2x2x2 / GEMM: four.  A fused tail fed split-pair activations (PS) uses the same stages: its slab lands
+// as [hi | lo] fp16 rows of the same 128 bytes and is read where it landed.
 // Every configuration stays within the 227 KB of shared memory an H100 block may use.  How many CTAs share an SM is set by
 // registers (tc_min_blocks below), not by shared memory.
 template <int BN, int KS, int ROWB, int X3 = 0, int N2 = 0>
@@ -225,11 +228,12 @@ struct TcStagesOf {
 };
 // CTAs per SM the kernel is compiled for (384 threads each): two for BN = 32, whose 16-register accumulators fit the 80
 // registers that leaves (one CTA's prologue / epilogue runs under the other's main loop), except the fp16-split 1x1, 2x2x2
-// and fused-tail kernels, which would spill or have their wgmmas serialized at 80 registers.  Every BN >= 64 kernel needs
-// more than 80 registers and runs one CTA per SM.
-template <int BN, int KS, int N2, int X3>
+// and fused-tail kernels that split their A operand in shared memory: the splitter warps' staging registers would spill or
+// have the wgmmas serialized at 80 registers.  The fused tail fed a pre-split A operand (PS) has no splitter and runs two
+// CTAs per SM (2 x 104-108 KB of shared memory).  Every BN >= 64 kernel needs more than 80 registers and runs one CTA per SM.
+template <int BN, int KS, int N2, int X3, bool PS = false>
 constexpr int tc_min_blocks() {
-    return (BN == 32 && !(X3 == 2 && (KS == 1 || KS == 2 || N2 > 0))) ? 2 : 1;
+    return (BN == 32 && (PS || !(X3 == 2 && (KS == 1 || KS == 2 || N2 > 0)))) ? 2 : 1;
 }
 template <int BN, int KS, int ROWB, int BY, int N2 = 0, int X3 = 0>
 constexpr size_t tc_smem_bytes() {
@@ -265,8 +269,15 @@ constexpr size_t tc_smem_bytes() {
 // buffer, the splitter warps write its hi and (scaled) lo parts as two fp16 K-major SWIZZLE_64B tiles, the weights are
 // pre-split fp16 tiles, and the three products are f16 wgmmas -- same 22 significand bits, twice the MMA rate.  The scaled
 // cross terms are a wgmma group of their own, folded into the running sum as fmaf(cross, 2^-11, sum).
-template <int BN, int KS, int EB = 4, int ROWB = 128, int BY = 2, int N2 = 0, int X3 = 0, int CL = 1>
-__global__ void __launch_bounds__(TC_THREADS, tc_min_blocks<BN, KS, N2, X3>()) conv3d_k3_tc_kernel(const __grid_constant__ CUtensorMap tmA,
+//
+// Split-pair activations (X3 = 2): [32 fp16 hi | 32 fp16 lo] per voxel and 32-channel slice, one 128-byte row, hi and lo
+// exactly as split_f16x2 makes them (the layout of the fp16-split weights).  The 1x1 kernel writes this format from its
+// post-bias / ReLU fp32 value when a.out_split is set; the fused tail with PS = true reads it as its A operand: the TMA box
+// {64 halves, 8 z, 2 y, 10 x} lands as SWIZZLE_128B rows, hi at +0 and lo at +64 -- the same descriptors as the weights --
+// so there are no splitter warps, no conv_done handoff and no proxy fence per stage.  The operand bits and the MMA order are
+// those of the fp32-input tail, so its result is bit-identical.
+template <int BN, int KS, int EB = 4, int ROWB = 128, int BY = 2, int N2 = 0, int X3 = 0, int CL = 1, bool PS = false>
+__global__ void __launch_bounds__(TC_THREADS, tc_min_blocks<BN, KS, N2, X3, PS>()) conv3d_k3_tc_kernel(const __grid_constant__ CUtensorMap tmA,
                                                                                   const __grid_constant__ CUtensorMap tmB,
                                                                                   const __grid_constant__ CUtensorMap tmB2,
                                                                                   const TcArgs a) {
@@ -274,7 +285,10 @@ __global__ void __launch_bounds__(TC_THREADS, tc_min_blocks<BN, KS, N2, X3>()) c
     static_assert(X3 == 0 || EB == 4, "3xTF32 splits fp32-stored operands");
     static_assert(X3 != 2 || ROWB == 128, "the fp16 split reads 128-byte fp32 rows and writes 64-byte fp16 rows");
     static_assert(CL == 1 || (CL == 2 && KS == 3), "weight-tile multicast: pairs of 3x3x3 bricks");
+    static_assert(!PS || (X3 == 2 && KS == 3 && N2 > 0 && CL == 1), "pre-split A operand: fp16-split fused tails");
     constexpr bool XH = X3 == 2;             // fp16 split
+    constexpr bool SPLITTER = X3 && !PS;     // warps 1-3 split the A slab in shared memory
+    constexpr int AOPB = PS ? 128 : (XH ? 64 : ROWB);  // bytes of one A operand row in shared memory (PS: [hi | lo] per row)
     constexpr bool F16 = EB == 2 || XH;      // f16 (else TF32) wgmma
     constexpr int NSPLIT = 96;               // splitter threads: warps 1-3
     constexpr int OPB = XH ? 64 : ROWB;      // bytes of one K-slice row of the MMA operands in shared memory
@@ -379,7 +393,8 @@ __global__ void __launch_bounds__(TC_THREADS, tc_min_blocks<BN, KS, N2, X3>()) c
                 if constexpr (X3 == 1) tma_load_2d(sa + B_OFF + B_BYTES, &tmB, full + s, tap * a.cin + kc * KC, a.cout + n0);
             } else {
                 const int dy = tap / 3, dz = tap % 3;  // tap = (dy, dz) pair; the slab covers x0-1 .. x0+8
-                tma_load_4d(sa, &tmA, full + s, kc * KC, z0 + dz - 1, y0 + dy - 1, x0 - 1);
+                // (PS: the channel coordinate counts halves, two per channel)
+                tma_load_4d(sa, &tmA, full + s, kc * KC * (PS ? 2 : 1), z0 + dz - 1, y0 + dy - 1, x0 - 1);
 #pragma unroll
                 for (int j = 0; j < NBT; ++j) {  // weight tiles: x-taps 0..2 (X3 = 1: hi tiles, then the low parts' tiles)
                     const int dx = j % 3, row0 = (j >= 3 ? a.cout : 0) + n0;
@@ -393,7 +408,7 @@ __global__ void __launch_bounds__(TC_THREADS, tc_min_blocks<BN, KS, N2, X3>()) c
                 }
             }
         }
-    } else if (X3 && warp >= 1 && warp <= 3) {
+    } else if (SPLITTER && warp >= 1 && warp <= 3) {
         // ===== operand splitter (warps 1-3) =====
         const int t = threadIdx.x - 32;
         for (int it = 0; it < total; ++it) {
@@ -455,10 +470,12 @@ __global__ void __launch_bounds__(TC_THREADS, tc_min_blocks<BN, KS, N2, X3>()) c
         for (int it = 0; it < total; ++it) {
             const int s = it % TC_STAGES;
             const uint32_t ph = (it / TC_STAGES) & 1;
-            mbar_wait(X3 ? conv_done + s : full + s, ph);  // X3: the split (which itself waited for the TMA) is done
+            mbar_wait(SPLITTER ? conv_done + s : full + s, ph);  // splitter: the split (which itself waited for the TMA) is done
             const uint32_t sa = smem_u32(smem + s * STAGE_BYTES), sb = sa + B_OFF;
-            // operand tiles: X3 = 1: hi at sa (in place), lo at sa + A_BYTES; X3 = 2: fp16 hi at sa (in place), lo half an A_BYTES on
-            const uint32_t a_hi = sa + row_off * OPB, a_lo = sa + (XH ? A_BYTES / 2 : A_BYTES) + row_off * OPB;
+            // operand tiles: X3 = 1: hi at sa (in place), lo at sa + A_BYTES; X3 = 2: fp16 hi at sa (in place), lo half an A_BYTES on;
+            // PS: [hi | lo] halves of each 128-byte row as landed
+            const uint32_t a_hi = sa + row_off * AOPB;
+            const uint32_t a_lo = PS ? a_hi + 64 : sa + (XH ? A_BYTES / 2 : A_BYTES) + row_off * OPB;
             float part[X3 ? BN / 2 : 1];  // X3: this stage's products (a fresh, short accumulation chain)
             // X3 = 1: one group, A_lo.B_hi + A_hi.B_lo + A_hi.B_hi (smallest terms first).  X3 = 2: the low parts are scaled by
             // 2^11, so the cross terms are a group of their own, added scaled back (pass 0), before the A_hi.B_hi group (pass 1)
@@ -468,11 +485,11 @@ __global__ void __launch_bounds__(TC_THREADS, tc_min_blocks<BN, KS, N2, X3>()) c
 #pragma unroll
                 for (int dx = 0; dx < XT; ++dx) {
                     // x-tap dx: A rows start 16 rows (= two 8-row swizzle atoms) further into the slab
-                    const uint32_t ax = a_hi + dx * (TC_BY * TC_BZ) * OPB, al_x = a_lo + dx * (TC_BY * TC_BZ) * OPB, bx = sb + dx * B_BYTES;
+                    const uint32_t ax = a_hi + dx * (TC_BY * TC_BZ) * AOPB, al_x = a_lo + dx * (TC_BY * TC_BZ) * AOPB, bx = sb + dx * B_BYTES;
 #pragma unroll
                     for (int k = 0; k < OPB / 32; ++k) {  // one MMA consumes 32 B of K (8 tf32 / 16 f16): advance inside the swizzle atom
                         if constexpr (X3) {
-                            const uint64_t ah = gmma_desc<OPB>(ax + k * 32), al = gmma_desc<OPB>(al_x + k * 32);
+                            const uint64_t ah = gmma_desc<AOPB>(ax + k * 32), al = gmma_desc<AOPB>(al_x + k * 32);
                             const uint64_t bh = gmma_desc<BROW>(bx + k * 32);
                             const uint64_t bl = XH ? gmma_desc<BROW>(bx + 64 + k * 32) : gmma_desc<BROW>(bx + XT * B_BYTES + k * 32);
                             if (pass == 0) {
@@ -567,7 +584,15 @@ __global__ void __launch_bounds__(TC_THREADS, tc_min_blocks<BN, KS, N2, X3>()) c
                 mbar_wait(b2_full, 0);
                 const uint32_t sa2 = smem_u32(a2) + row_off * (XH ? 64 : 128), sb2 = smem_u32(smem_b2);
                 constexpr int OP2 = XH ? 64 : 128;
-                float cross[XH ? N2 / 2 : 1];  // X3 = 2: the cross terms (scaled by 2^11), added scaled back after the hi.hi group
+                // X3 = 2: the cross terms (scaled by 2^11), added scaled back after the hi.hi group.  A kernel compiled for two
+                // CTAs per SM (80 registers) cannot hold two N2 = 64 accumulators, so it parks the cross terms in the drained
+                // stages behind A2, one column-major block per warpgroup (thread tw's i-th value at [i][tw]: no bank conflicts).
+                // Like A2 this relies on the kernel handling one brick: once the main loop is over no TMA is in flight, so the
+                // stages are free (a schedule that prefetched the next brick's slabs here would need its own space)
+                constexpr bool STASH = XH && N2 > 32 && tc_min_blocks<BN, KS, N2, X3, PS>() == 2;
+                static_assert(!STASH || 2 * A2_BYTES + 2 * (N2 / 2) * 128 * 4 <= TC_STAGES * STAGE_BYTES, "stash fits the stages");
+                float cross[XH && !STASH ? N2 / 2 : 1];
+                float *stash = reinterpret_cast<float *>(smem + 2 * A2_BYTES) + wg * (N2 / 2) * 128 + tw;
 #pragma unroll
                 for (int pass = 0; pass < (XH ? 2 : 1); ++pass) {
                     wgmma_fence();
@@ -595,10 +620,13 @@ __global__ void __launch_bounds__(TC_THREADS, tc_min_blocks<BN, KS, N2, X3>()) c
                     if constexpr (XH) {
                         if (pass == 0) {
 #pragma unroll
-                            for (int i = 0; i < N2 / 2; ++i) cross[i] = acc2[i];
+                            for (int i = 0; i < N2 / 2; ++i) {
+                                if constexpr (STASH) stash[i * 128] = acc2[i];
+                                else cross[i] = acc2[i];
+                            }
                         } else {
 #pragma unroll
-                            for (int i = 0; i < N2 / 2; ++i) acc2[i] = fmaf(cross[i], 1.0f / 2048.0f, acc2[i]);
+                            for (int i = 0; i < N2 / 2; ++i) acc2[i] = fmaf(STASH ? stash[i * 128] : cross[i], 1.0f / 2048.0f, acc2[i]);
                         }
                     }
                 }
@@ -614,6 +642,8 @@ __global__ void __launch_bounds__(TC_THREADS, tc_min_blocks<BN, KS, N2, X3>()) c
                 float *orow = a.out ? a.out + vox * a.out_ld + a.out_coff + n0 : nullptr;
                 __half *hrow = a.out16 ? a.out16 + vox * a.out_ld + a.out_coff + n0 : nullptr;
                 const float *rrow = a.res ? a.res + vox * a.res_ld + a.res_coff + n0 : nullptr;
+                __half *srow = nullptr;  // split-pair row of this voxel (channel c at (c / 32) * 64 + c % 32, its lo 32 halves on)
+                if constexpr (XH && KS == 1) srow = a.out_split ? a.out_split + vox * 2 * a.cout + 2 * n0 : nullptr;
 #pragma unroll
                 for (int j = 0; j < NOUT / 8; ++j) {
                     const int c = 8 * j + 2 * q;
@@ -629,6 +659,15 @@ __global__ void __launch_bounds__(TC_THREADS, tc_min_blocks<BN, KS, N2, X3>()) c
                     if (a.act == 1) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
                     if (orow) *reinterpret_cast<float2 *>(orow + c) = o;
                     if (hrow) *reinterpret_cast<__half2 *>(hrow + c) = __floats2half2_rn(o.x, o.y);
+                    if constexpr (XH && KS == 1) {
+                        if (srow) {
+                            uint32_t hi, lo;
+                            split_f16x2(o.x, o.y, hi, lo);
+                            __half *p = srow + (c >> 5) * 64 + (c & 31);
+                            *reinterpret_cast<uint32_t *>(p) = hi;
+                            *reinterpret_cast<uint32_t *>(p + 32) = lo;
+                        }
+                    }
                 }
             }
         }
@@ -704,11 +743,11 @@ static EncodeTiledFn get_encode() {
     return fn;
 }
 
-template <int BN, int KS, int EB = 4, int ROWB = 128, int BY = 2, int N2 = 0, int X3 = 0, int CL = 1>
+template <int BN, int KS, int EB = 4, int ROWB = 128, int BY = 2, int N2 = 0, int X3 = 0, int CL = 1, bool PS = false>
 static int launch_tc(const CUtensorMap &tmA, const CUtensorMap &tmB, const TcArgs &a_in, int n_tiles, cudaStream_t s,
                      const CUtensorMap *tmB2 = nullptr, int grid_z = 1) {
     const size_t smem = tc_smem_bytes<BN, KS, ROWB, BY, N2, X3>();
-    auto kern = conv3d_k3_tc_kernel<BN, KS, EB, ROWB, BY, N2, X3, CL>;
+    auto kern = conv3d_k3_tc_kernel<BN, KS, EB, ROWB, BY, N2, X3, CL, PS>;
     static bool attr_done = false;
     if (!attr_done) {
         if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
@@ -798,8 +837,10 @@ static bool use_cluster() {
 
 static int conv3d_k3_tc_impl(const float *in, const float *w_tc, const float *bias, const float *residual, int res_ld,
                              int res_coff, float *out, int out_ld, int out_coff, int X, int Y, int Z, int cin, int cout,
-                             int ks, const int32_t *tiles, int n_tiles, int act, void *stream, int x3) {
-    if (!in || !w_tc || !out || X <= 0 || Y <= 0 || Z <= 0 || (ks != 1 && ks != 2 && ks != 3)) return SIS3D_EINVAL;
+                             int ks, const int32_t *tiles, int n_tiles, int act, void *stream, int x3,
+                             __half *out_split = nullptr) {
+    if (!in || !w_tc || !(out || out_split) || X <= 0 || Y <= 0 || Z <= 0 || (ks != 1 && ks != 2 && ks != 3)) return SIS3D_EINVAL;
+    if (out_split && (x3 != 2 || ks != 1 || cout % TC_KC || ((uintptr_t)out_split & 15))) return SIS3D_EINVAL;
     if (ks == 2 && (tiles || X < 2 || Y < 2 || Z < 2)) return SIS3D_EINVAL;
     if (x3 && tiles) return SIS3D_EUNSUPPORTED;  // the ragged mask stage does not need the compensated product
     const int taps = ks * ks * ks;
@@ -842,7 +883,7 @@ static int conv3d_k3_tc_impl(const float *in, const float *w_tc, const float *bi
             return SIS3D_EINVAL;
     }
     TcArgs a;
-    a.bias = bias; a.res = residual; a.out = out; a.tiles = tiles; a.out16 = nullptr; a.bias_mid = nullptr;
+    a.bias = bias; a.res = residual; a.out = out; a.tiles = tiles; a.out16 = nullptr; a.bias_mid = nullptr; a.out_split = out_split;
     a.X = Xo; a.Y = Yo; a.Z = Zo; a.cin = cin; a.cout = cout; a.act = act;
     a.out_ld = out_ld; a.out_coff = out_coff; a.res_ld = res_ld; a.res_coff = res_coff;
     a.tiles_y = cdiv(Yo, by); a.tiles_z = cdiv(Zo, TC_BZ);
@@ -934,6 +975,13 @@ extern "C" int sis3d_conv3d_k3_tc_h3(const float *in, const uint16_t *w_h3, cons
     return conv3d_k3_tc_impl(in, (const float *)w_h3, bias, residual, res_ld, res_coff, out, out_ld, out_coff, X, Y, Z, cin, cout,
                              ks, nullptr, 0, act, stream, 2);
 }
+// the fp16-split 1x1 conv writing split-pair activations (the A operand of sis3d_conv3d_k3_tc_fused_h3_split) instead of fp32
+extern "C" int sis3d_conv3d_k1_tc_h3_split(const float *in, const uint16_t *w_h3, const float *bias, uint16_t *out_split, int X,
+                                           int Y, int Z, int cin, int cout, int act, void *stream) {
+    if (!out_split) return SIS3D_EINVAL;
+    return conv3d_k3_tc_impl(in, (const float *)w_h3, bias, nullptr, 0, 0, nullptr, cout, 0, X, Y, Z, cin, cout, 1, nullptr, 0, act,
+                             stream, 2, (__half *)out_split);
+}
 
 // ---- bottleneck tail: 3x3x3 conv (cin -> cmid) + ReLU + 1x1 conv (cmid -> cout) + residual + act, one kernel ----------------
 extern "C" int sis3d_conv3d_k3_tc_fused_supported(int cin, int cmid, int cout) {
@@ -942,8 +990,9 @@ extern "C" int sis3d_conv3d_k3_tc_fused_supported(int cin, int cmid, int cout) {
 static int conv3d_k3_tc_fused_impl(const float *in, const float *w2_tc, const float *bias2, const float *w3_tc,
                                    const float *bias3, const float *residual, int res_ld, int res_coff, float *out,
                                    int out_ld, int out_coff, int X, int Y, int Z, int cin, int cmid, int cout, int act,
-                                   void *stream, int x3) {
+                                   void *stream, int x3, bool presplit = false) {
     if (!in || !w2_tc || !w3_tc || !out || X <= 0 || Y <= 0 || Z <= 0) return SIS3D_EINVAL;
+    if (presplit && x3 != 2) return SIS3D_EINVAL;
     if (!sis3d_conv3d_k3_tc_fused_supported(cin, cmid, cout)) return SIS3D_EUNSUPPORTED;
     if (((uintptr_t)in | (uintptr_t)w2_tc | (uintptr_t)w3_tc | (uintptr_t)out) & 15) return SIS3D_EINVAL;
     if ((out_ld | out_coff | res_ld | res_coff) & 3) return SIS3D_EINVAL;
@@ -961,11 +1010,14 @@ static int conv3d_k3_tc_fused_impl(const float *in, const float *w2_tc, const fl
     CUtensorMap tmA, tmB, tmB2;
     cuuint32_t estr[4] = {1, 1, 1, 1};
     {
-        cuuint64_t dims[4] = {(cuuint64_t)cin, (cuuint64_t)Z, (cuuint64_t)Y, (cuuint64_t)X};
+        // presplit: split-pair fp16 rows, 2 cin halves per voxel (4 bytes per channel, the byte strides of fp32); a box row of
+        // 64 halves = one 32-channel slice's [hi | lo]
+        cuuint64_t dims[4] = {(cuuint64_t)cin * (presplit ? 2 : 1), (cuuint64_t)Z, (cuuint64_t)Y, (cuuint64_t)X};
         cuuint64_t strides[3] = {(cuuint64_t)cin * 4, (cuuint64_t)Z * cin * 4, (cuuint64_t)Y * Z * cin * 4};
-        cuuint32_t box[4] = {(cuuint32_t)kc, TC_BZ, (cuuint32_t)by, (cuuint32_t)(bx + 2)};
-        if (enc(&tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void *)in, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+        cuuint32_t box[4] = {(cuuint32_t)(presplit ? 2 * TC_KC : kc), TC_BZ, (cuuint32_t)by, (cuuint32_t)(bx + 2)};
+        if (enc(&tmA, presplit ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void *)in, dims, strides, box,
+                estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) !=
+            CUDA_SUCCESS)
             return SIS3D_EINVAL;
     }
     {
@@ -985,7 +1037,7 @@ static int conv3d_k3_tc_fused_impl(const float *in, const float *w2_tc, const fl
             return SIS3D_EINVAL;
     }
     TcArgs a;
-    a.bias = bias3; a.bias_mid = bias2; a.res = residual; a.out = out; a.tiles = nullptr; a.out16 = nullptr;
+    a.bias = bias3; a.bias_mid = bias2; a.res = residual; a.out = out; a.tiles = nullptr; a.out16 = nullptr; a.out_split = nullptr;
     // the main loop's weight rows (and their lo halves, x3) are indexed with the 3x3x3 conv's width, the epilogue with cout
     a.X = X; a.Y = Y; a.Z = Z; a.cin = cin; a.cout = x3 ? cmid : cout; a.act = act;
     a.out_ld = out_ld; a.out_coff = out_coff; a.res_ld = res_ld; a.res_coff = res_coff;
@@ -993,6 +1045,11 @@ static int conv3d_k3_tc_fused_impl(const float *in, const float *w2_tc, const fl
     a.gemm_m = 0; a.gemm_chunks_per_split = 0;
     const int n_tiles = cdiv(X, bx) * a.tiles_y * a.tiles_z;
     cudaStream_t s = (cudaStream_t)stream;
+    if (presplit) {
+        if (cmid == 32 && cout == 32) return launch_tc<32, 3, 4, 128, 2, 32, 2, 1, true>(tmA, tmB, a, n_tiles, s, &tmB2);
+        if (cmid == 32 && cout == 64) return launch_tc<32, 3, 4, 128, 2, 64, 2, 1, true>(tmA, tmB, a, n_tiles, s, &tmB2);
+        return launch_tc<64, 3, 4, 128, 2, 128, 2, 1, true>(tmA, tmB, a, n_tiles, s, &tmB2);
+    }
     if (x3 == 2) {
         if (cmid == 32 && cout == 32) return launch_tc<32, 3, 4, 128, 2, 32, 2>(tmA, tmB, a, n_tiles, s, &tmB2);
         if (cmid == 32 && cout == 64) return launch_tc<32, 3, 4, 128, 2, 64, 2>(tmA, tmB, a, n_tiles, s, &tmB2);
@@ -1028,6 +1085,14 @@ extern "C" int sis3d_conv3d_k3_tc_fused_h3(const float *in, const uint16_t *w2_h
                                            void *stream) {
     return conv3d_k3_tc_fused_impl(in, (const float *)w2_h3, bias2, (const float *)w3_h3, bias3, residual, res_ld, res_coff, out,
                                    out_ld, out_coff, X, Y, Z, cin, cmid, cout, act, stream, 2);
+}
+// the same tail fed split-pair activations (from sis3d_conv3d_k1_tc_h3_split): no operand split on the SM, same result bits
+extern "C" int sis3d_conv3d_k3_tc_fused_h3_split(const uint16_t *in_split, const uint16_t *w2_h3, const float *bias2,
+                                                 const uint16_t *w3_h3, const float *bias3, const float *residual, int res_ld,
+                                                 int res_coff, float *out, int out_ld, int out_coff, int X, int Y, int Z, int cin,
+                                                 int cmid, int cout, int act, void *stream) {
+    return conv3d_k3_tc_fused_impl((const float *)in_split, (const float *)w2_h3, bias2, (const float *)w3_h3, bias3, residual,
+                                   res_ld, res_coff, out, out_ld, out_coff, X, Y, Z, cin, cmid, cout, act, stream, 2, true);
 }
 
 // ---- y[M][N] = act(x[M][K] . w[N][K]^T + b): fully connected layer on the tensor cores (TF32), split-K ------------

@@ -512,11 +512,33 @@ class Network(nn.Module):
         """1x1 -> relu -> 3x3x3 -> relu -> 1x1 (+x) -> relu  (reference: backbones.py:28-40).  In 'fp16' math the two inner
         activations exist only as fp16 (they feed tensor-core layers only); the block output is fp32 (+ fp16 twin when it
         is a dense tensor, for the next block's first conv)."""
-        y = self._conv(x, name + ".conv1", act=1, want32=False, want16=True)
-        n2, n3 = name + ".conv2", name + ".conv3"
+        n1, n2, n3 = name + ".conv1", name + ".conv2", name + ".conv3"
         x3 = self._math in ("tf32x3", "f16x3")
         h3 = self._math == "f16x3"
         wt = self._packed_h3 if h3 else (self._packed_x3 if x3 else self._packed_tc)
+        if (h3 and self._fuse_bneck and n1 in wt and n2 in wt and n3 in wt and x.t is not None and x.layout == "vc"
+                and x.ld == x.C and x.coff == 0):
+            _, b1, c1, cin1, ks1 = self._packed[n1]
+            _, _, cmid, cin, _ = self._packed[n2]
+            cout = self._packed[n3][2]
+            if ks1 == 1 and cin1 == x.C and c1 == cin and S.lib.sis3d_conv3d_k3_tc_fused_supported(cin, cmid, cout):
+                # conv1 writes its activation already split into fp16 hi / lo pairs, the form the tail's MMAs read: the tail
+                # needs no operand split on the SM (the result bits are those of the fp32 hand-off below)
+                ys = torch.empty(*x.dims, 2 * c1, dtype=torch.float16, device=x.t.device)
+                tok = self._rec(f"conv_tc_h3_split[{n1}]")
+                S.check(S.lib.sis3d_conv3d_k1_tc_h3_split(S.ptr(x.t), S.ptr(wt[n1]), S.ptr(b1), S.ptr(ys), *x.dims, cin1, c1, 1,
+                                                          S.stream()), f"conv3d_k1_tc_h3_split[{n1}]")
+                self._rec_end(tok)
+                if out is None:
+                    out = Act(torch.empty(*x.dims, cout, dtype=torch.float32, device=x.t.device), x.dims, cout)
+                tok = self._rec(f"conv_tc_fused_h3_split[{name}]")
+                S.check(S.lib.sis3d_conv3d_k3_tc_fused_h3_split(
+                    S.ptr(ys), S.ptr(wt[n2]), S.ptr(self._packed[n2][1]), S.ptr(wt[n3]), S.ptr(self._packed[n3][1]), S.ptr(x.t),
+                    x.ld, x.coff, S.ptr(out.t), out.ld, out.coff, *x.dims, cin, cmid, cout, 1, S.stream()),
+                    f"conv3d_k3_tc_fused_h3_split[{name}]")
+                self._rec_end(tok)
+                return out
+        y = self._conv(x, n1, act=1, want32=False, want16=True)
         if self._math in ("tf32", "tf32x3", "f16x3") and self._fuse_bneck and n2 in wt and n3 in wt and y.t is not None:
             _, _, cmid, cin, _ = self._packed[n2]
             cout = self._packed[n3][2]

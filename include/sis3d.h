@@ -232,6 +232,19 @@ int sis3d_conv3d_k3_tc_fused_h3(const float *in, const uint16_t *w2_h3, const fl
                                 void *stream);
 int sis3d_linear_tc_h3(const float *x, const uint16_t *w_h3, const float *bias, float *y, int M, int K, int N, int act,
                        void *workspace, size_t workspace_bytes, void *stream);
+/* Split-pair activations: the fp16 split done once, by the layer that produces the activation.  Per voxel and 32-channel
+ * slice one 128-byte row of 32 hi halves = fp16(v) followed by 32 lo halves = fp16((v - hi) * 2048) (the layout of the _h3
+ * weights): a dense VC tensor of 2 * C halves per voxel, 4 bytes per channel like fp32.
+ * sis3d_conv3d_k1_tc_h3_split: the 1x1 conv of sis3d_conv3d_k3_tc_h3 (ks = 1, no residual, cout % 32 == 0) writing out_split
+ * in this format from the same post-bias / activation fp32 value.
+ * sis3d_conv3d_k3_tc_fused_h3_split: sis3d_conv3d_k3_tc_fused_h3 reading its input in this format; the result is
+ * bit-identical to the fp32-input entry point on the fp32 tensor the split was made from. */
+int sis3d_conv3d_k1_tc_h3_split(const float *in, const uint16_t *w_h3, const float *bias, uint16_t *out_split, int X, int Y,
+                                int Z, int cin, int cout, int act, void *stream);
+int sis3d_conv3d_k3_tc_fused_h3_split(const uint16_t *in_split, const uint16_t *w2_h3, const float *bias2,
+                                      const uint16_t *w3_h3, const float *bias3, const float *residual, int res_ld,
+                                      int res_coff, float *out, int out_ld, int out_coff, int X, int Y, int Z, int cin,
+                                      int cmid, int cout, int act, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * fp16-operand tensor-core path (f16 wgmma, fp32 accumulate): activations and weights are STORED as fp16 (same
