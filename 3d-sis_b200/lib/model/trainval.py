@@ -57,10 +57,68 @@ def save_scene_results(out_dir, scene_id, blobs, net_or_predictions):
     return d
 
 
-def run_scenes(net, data_loader, out_dir, skip_existing=False, pipelined=True):
+class SceneEvaluator:
+    """Box and mask mAP of test mode (SolverWrapper.test, trainval.py:775-776, 844-845, 847-921, 926-941), fed one scene at
+    a time by run_scenes.  The box IoU and the matching run on the host.  The mask overlaps are counted on the device from
+    the mask stage's thresholded bits (lib.utils.evaluation.launch_mask_overlap); the counts of a scene are collected when
+    the next scene is added, so the scene loop never waits for them."""
+
+    def __init__(self):
+        from lib.utils.evaluation import DetectionMAP
+        self.box = DetectionMAP(cfg.NUM_CLASSES, ignore_class=[0], overlap_threshold=cfg.MAP_THRESH)
+        self.mask = DetectionMAP(cfg.NUM_CLASSES, ignore_class=[0], overlap_threshold=cfg.MAP_THRESH)
+        self._pending = None
+
+    def add(self, scene_dir, blobs, P):
+        """One scene: writes gt_class.npy / gt_box.npy (and the pickled gt_mask) beside its predictions, accumulates the box
+        mAP of the kept detections and queues the mask overlaps of the kept masks."""
+        from lib.utils.evaluation import launch_mask_overlap, pack_masks
+        gt = blobs["gt_box"][0].numpy()
+        gt_box, gt_class = gt[:, 0:6], gt[:, 6]
+        np.save(os.path.join(scene_dir, "gt_class"), gt_class)
+        np.save(os.path.join(scene_dir, "gt_box"), gt_box)
+        pred_class, pred_conf, pred_box, keep = detections_from_predictions(P)
+        self.box.evaluate(pred_box[keep], pred_class[keep], pred_conf[keep], gt_box, gt_class)
+        if not cfg.USE_MASK:
+            return
+        gt_mask = blobs["gt_mask"][0]
+        with open(os.path.join(scene_dir, "gt_mask"), "wb") as f:
+            pickle.dump(gt_mask, f)
+        dims = tuple(int(v) for v in blobs["data"].shape[2:])  # the reference's net._scene_info
+        gb, go, gbox = pack_masks(gt_mask, gt_box, dims, "GT")
+        det = P["detections_host"]
+        if "mask_bits" in P:  # crop i of the packed bits sits at the crop bounds of kept detection i (columns 9-14)
+            job = launch_mask_overlap(P["mask_bits"], P["mask_offsets"], det[keep][:, 9:15], gb, go, gbox)
+        else:                 # no kept detection
+            job = launch_mask_overlap(np.zeros(0, np.uint8), np.zeros(0, np.int64), np.zeros((0, 6), np.int32), gb, go, gbox)
+        self._collect()
+        self._pending = (job, pred_class[keep], pred_conf[keep], gt_class)
+
+    def _collect(self):
+        if self._pending is not None:
+            job, pred_class, pred_conf, gt_class = self._pending
+            self._pending = None
+            self.mask.evaluate_overlaps(pred_class, pred_conf, job.result(), gt_class)
+
+    def summary(self):
+        """Collects the last scene and returns the lines test mode prints (trainval.py:929-941)."""
+        from lib.utils.evaluation import summary_lines
+        self._collect()
+        lines = []
+        if cfg.USE_CLASS:
+            self.box.finalize()
+            lines += summary_lines("CLASSIFICATION", self.box, int(cfg.NUM_CLASSES))
+        if cfg.USE_MASK:
+            self.mask.finalize()
+            lines += summary_lines("mask", self.mask, int(cfg.NUM_CLASSES))
+        return lines
+
+
+def run_scenes(net, data_loader, out_dir, skip_existing=False, pipelined=True, evaluator=None):
     """The scene loop of SolverWrapper.test / .benchmark (trainval.py:787-911).  pipelined=True drives it through
     Network.forward_pipelined (several scenes in flight, results read back asynchronously); blobs that carry precomputed
-    projection index lists (the reference's calling convention) go through the synchronous forward."""
+    projection index lists (the reference's calling convention) go through the synchronous forward.  An `evaluator`
+    (SceneEvaluator) is handed every scene after its result files are written."""
     os.makedirs(out_dir, exist_ok=True)
     t0 = time.time()
     done = 0
@@ -76,7 +134,9 @@ def run_scenes(net, data_loader, out_dir, skip_existing=False, pipelined=True):
         if first is not None and "proj_ind_3d" not in first:
             import itertools
             for blobs, P in net.forward_pipelined(itertools.chain([first], it)):
-                save_scene_results(out_dir, blobs["id"][0], blobs, P)
+                d = save_scene_results(out_dir, blobs["id"][0], blobs, P)
+                if evaluator is not None:
+                    evaluator.add(d, blobs, P)
                 done += 1
             it = iter(())
         elif first is not None:
@@ -84,7 +144,9 @@ def run_scenes(net, data_loader, out_dir, skip_existing=False, pipelined=True):
             it = itertools.chain([first], it)
     for blobs in it:
         net.forward(blobs, "TEST", None)
-        save_scene_results(out_dir, blobs["id"][0], blobs, net)
+        d = save_scene_results(out_dir, blobs["id"][0], blobs, net)
+        if evaluator is not None:
+            evaluator.add(d, blobs, net._predictions)
         done += 1
     torch.cuda.synchronize()
     print("It took {:.3f}s for test on whole scenes".format(time.time() - t0))
@@ -109,9 +171,15 @@ def _build(args, mode, view_provider=None):
     return net, loader
 
 
-def test(args, view_provider=None):
+def test(args, view_provider=None, pipelined=True):
+    """Every scene's result files plus gt_class.npy, gt_box.npy and the pickled gt_mask, then the reference's box and mask
+    mAP summary (trainval.py:926-941) on stdout."""
     net, loader = _build(args, "test", view_provider)
-    return run_scenes(net, loader, cfg.TEST_SAVE_DIR)
+    ev = SceneEvaluator()
+    done = run_scenes(net, loader, cfg.TEST_SAVE_DIR, pipelined=pipelined, evaluator=ev)
+    for line in ev.summary():
+        print(line)
+    return done
 
 
 def benchmark(args, view_provider=None):

@@ -25,7 +25,7 @@ def _defaults():
     c = AttrDict()
     c.TEST = AttrDict(RPN_NMS_THRESH=0.35, RPN_PRE_NMS_TOP_N=6000, RPN_POST_NMS_TOP_N=300)
     c.TRAIN = AttrDict(RPN_NMS_THRESH=0.7, RPN_PRE_NMS_TOP_N=12000, RPN_POST_NMS_TOP_N=2000)
-    c.update(ALLOW_BORDER=0, RPN_CHANNELS=256, CLASS_POOLING_SIZE=2, CLASS_THRESH=0.9, MASK_THRESH=0.5,
+    c.update(ALLOW_BORDER=0, RPN_CHANNELS=256, CLASS_POOLING_SIZE=2, CLASS_THRESH=0.9, MASK_THRESH=0.5, MAP_THRESH=0.25,
              MASK_USE_IMAGES=False, MASK_ONLY_IMAGES=False, MAX_IMAGE=400, MAX_VOLUME=2000000,
              NUM_CLASSES=0, BATCH_SIZE=1, VOXEL_SIZE=0.09375, TRUNCATED=3.0,
              NUM_ANCHORS_LEVEL1=9, NUM_ANCHORS_LEVEL2=9, NUM_ANCHORS_LEVEL3=9,

@@ -276,6 +276,33 @@ def make_net(c, keep_debug=True, math="fp32", weights=None, enet=False):
     return net, cfg
 
 
+def write_chunks(out_dir, c, seeds, label_seed=5):
+    """Synthetic .chunk files of a case with GT for test mode's mAP: boxes from make_scene with random labels 1..18, each GT mask
+    the voxels of negative SDF inside the box's floor / ceil bounds (as the dataset rounds it).  -> (paths, view_provider)."""
+    import os
+    from lib.datasets.scene_io import write_scene
+    paths, provs = [], {}
+    rng = np.random.default_rng(label_seed)
+    for k, seed in enumerate(seeds):
+        data, boxes = make_scene(seed, c["dims"])
+        views = make_views(seed, c["dims"], c["n_img"], boxes)
+        sdf = np.where(data[0, 1] > 0.5, data[0, 0], -data[0, 0]).astype(np.float32)
+        sdf[(data[0, 1] < 0.5) & (data[0, 0] < 1.0)] = -1.0
+        gt, masks = [], []
+        for b in boxes:
+            lo, hi = np.floor(b[:3]).astype(int), np.ceil(b[3:]).astype(int)
+            label = int(rng.integers(1, 19))
+            gt.append(list(b) + [label])
+            masks.append((label, (sdf[lo[0]:hi[0], lo[1]:hi[1], lo[2]:hi[2]] < 0).astype(np.uint16)))
+        p = os.path.join(out_dir, f"scene{k:04d}_00__0.chunk")
+        write_scene(p, sdf, np.array(gt, np.float32), masks, world2grid=views["world2grid"], frame_ids=[0, 20, 40])
+        paths.append(p)
+        provs[p] = views
+    provider = lambda p, ids, w2g, dims: {"images": provs[p]["feats"], "depths": provs[p]["depths"], "poses": provs[p]["poses"],
+                                          "world2grid": provs[p]["world2grid"]}
+    return paths, provider
+
+
 def make_blobs(c, data, views, pin=False):
     """The reference's blob dict (lib/datasets/dataloader.py collate_fn) for one synthetic scene."""
     import torch

@@ -358,6 +358,23 @@ int sis3d_memcpy_async(void *dst, const void *src, size_t bytes, int kind, void 
 int sis3d_mask_select(const float *masks, const int64_t *offs, const int32_t *cls, int n_crops, int ncls,
                       int64_t total_hint, float thresh, float *out, uint8_t *bits, void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Voxel overlaps of predicted and GT instance masks for the mask mAP of test mode.  Replaces the
+ * full-scene unmold_mask + jaccard_mask of lib/utils/evaluation.py:144-179, 293-307.
+ * Each mask is packed uint8, C order [w][h][l], at its box: *_bits + *_offs[i] (int64 offsets, one per
+ * mask), *_box int32[n][6] = lo xyz | hi xyz (hi exclusive, extent = the mask's shape).  The predicted
+ * side is the mask stage's `bits` with the crop bounds of sis3d_detect_decode (columns 9-14).
+ * pairs int32[n_pairs][2] = (prediction, GT) indices; only the intersection of the two boxes is visited,
+ * so list the pairs whose boxes intersect (the others have no common voxel).
+ * Outputs (exact int64 counts of nonzero voxels): pred_count[n_pred], gt_count[n_gt],
+ * pair_count[n_pairs] (voxels nonzero in both masks; -1 for a pair index out of range).
+ * One launch, no workspace, capturable in a CUDA graph.
+ * ---------------------------------------------------------------------------------------------- */
+int sis3d_mask_overlap(const uint8_t *pred_bits, const int64_t *pred_offs, const int32_t *pred_box, int n_pred,
+                       const uint8_t *gt_bits, const int64_t *gt_offs, const int32_t *gt_box, int n_gt,
+                       const int32_t *pairs, int n_pairs, int64_t *pred_count, int64_t *gt_count,
+                       int64_t *pair_count, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
