@@ -31,3 +31,10 @@ template <class T> inline T atomicMax(T *p, T v) {
     while (old < v && !__atomic_compare_exchange_n(p, &old, v, true, __ATOMIC_RELAXED, __ATOMIC_RELAXED)) {}
     return old;
 }
+template <class T> inline T atomicMin(T *p, T v) {
+    T old = __atomic_load_n(p, __ATOMIC_RELAXED);
+    while (v < old && !__atomic_compare_exchange_n(p, &old, v, true, __ATOMIC_RELAXED, __ATOMIC_RELAXED)) {}
+    return old;
+}
+inline double __dmul_rn(double a, double b) { volatile double r = a * b; return r; }
+inline double __dadd_rn(double a, double b) { volatile double r = a + b; return r; }

@@ -8,11 +8,20 @@ file export, not the GPU hot path).
 
 Deviations, on purpose: vertices that land outside the volume (or whose neighbourhood would leave it) are skipped;
 the reference indexes the array with them (IndexError, or a silent wrap-around for -1).
+
+    python vox2mesh.py --pred_dir RESULTS --scan_path SCANS --frames FRAMES [--output_dir DIR]
+
+runs the reference's command line (vox2mesh.py:123-145): for every result folder `<scene>` of `pred_dir` with a mesh
+`<scan_path>/<scene>/<scene>_vh_clean_2.ply`, it reads the mesh and `<frames>/<scene>/world2grid.txt`, paints the
+predictions and writes `<scene>.txt` plus `predicted_masks/` into `output_dir`, the input of evaluate_semantic_instance.py.
+Folders are visited in sorted order; folders without a mesh are skipped.
 """
 from __future__ import annotations
 
+import argparse
 import os
 import pickle
+import sys
 
 import numpy as np
 
@@ -133,3 +142,37 @@ def load_matrix(filename):
             matrix[ind, :3] = [float(parts[0]), float(parts[1]), float(parts[2])]
             matrix[ind, 3] = float(parts[3]) - padding[ind]
     return matrix
+
+
+def main(argv=None):
+    """vox2mesh.py:123-145: every result folder with a mesh -> benchmark files in --output_dir."""
+    if __package__:
+        from . import utils
+    else:  # run as a script
+        import utils
+    parser = argparse.ArgumentParser()
+    parser.add_argument("--pred_dir", required=True, help="benchmark-mode result folders, one per scene")
+    parser.add_argument("--output_dir", default="./ScanNet_Benchmark_Result", help="output directory")
+    parser.add_argument("--scan_path", required=True, help="ScanNet scans: <scene>/<scene>_vh_clean_2.ply")
+    parser.add_argument("--frames", required=True, help="frames folders: <scene>/world2grid.txt")
+    opt = parser.parse_args(argv)
+    names = sorted(os.listdir(opt.pred_dir))
+    for ind, name in enumerate(names):
+        print("{}/{}".format(ind, len(names)))
+        mesh_file = os.path.join(opt.scan_path, name, name + "_vh_clean_2.ply")
+        if not os.path.isdir(os.path.join(opt.pred_dir, name)) or not os.path.exists(mesh_file):
+            continue
+        os.makedirs(opt.output_dir, exist_ok=True)
+        world2grid = load_matrix(os.path.join(opt.frames, name, "world2grid.txt"))
+        mesh_vertices = utils.read_mesh_vertices(mesh_file)
+        folder = os.path.join(opt.pred_dir, name)
+        with open(os.path.join(folder, "pred_mask_index"), "rb") as f:
+            kept = len(pickle.load(f))
+        # a scene without detections paints nothing (load_pred cannot index with an empty list)
+        scene = load_pred(folder) if kept else np.zeros(SCENE_DIMS)
+        export(mesh_vertices, world2grid, scene, opt.output_dir, name)
+        sys.stdout.flush()
+
+
+if __name__ == "__main__":
+    main()

@@ -375,6 +375,36 @@ int sis3d_mask_overlap(const uint8_t *pred_bits, const int64_t *pred_offs, const
                        const int32_t *pairs, int n_pairs, int64_t *pred_count, int64_t *gt_count,
                        int64_t *pair_count, void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * ScanNet benchmark: voxel instances -> mesh vertices -> per-(box, GT id) vertex counts, without the
+ * painted float64 canvas or per-vertex text files (tools/scannet_benchmark/vox2mesh.py:40-108 of the
+ * reference, tools/scannet_benchmark/evaluate_predictions.py here).
+ *
+ * sis3d_instance_paint: owner volume int32 [X][Y][Z] (C order) over the canvas voxels [x0, x0+X) x
+ * [y0, y0+Y) x [z0, z0+Z).  owner = the smallest box index b whose mask covers the voxel, -1 if none
+ * ("first box wins"; vox2mesh's painting order).  Masks in the sis3d_mask_overlap layout: bits +
+ * offs[b], box int32[n_box][6] = lo | hi in canvas voxels (hi exclusive, extent = the mask's shape); a
+ * box with hi <= lo on any axis paints nothing.  One launch.
+ *
+ * sis3d_vertex_instance_overlap: per vertex v (float32 xyz), g = rint(world2grid . [v, 1]) in fp64
+ * (row r: ((w[r][0]*x + w[r][1]*y) + w[r][2]*z) + w[r][3], each operation rounded, no FMA).  If
+ * 1 <= g <= canvas - 2 on every axis, the vertex takes the owner at g, else the first owned voxel of
+ * g's 3x3x3 neighbourhood in (dx, dy, dz) order, dx slowest, each in -1, 0, 1 (vox2mesh nn_search).
+ * Voxels outside the owner volume are unowned.  Outputs, for vertices that take a box b < n_box:
+ * hist int64[n_box][n_slot] += 1 at [b][gt_slot[v]] (slots outside [0, n_slot) are not counted),
+ * first_vertex int32[n_box] = the smallest such v (INT32_MAX for a box no vertex takes), and, when
+ * vertex_box is not NULL, vertex_box int32[n_vert] = b or -1.  hist and first_vertex are initialised
+ * by the call.  world2grid: 16 doubles, row major, on the device.  Two launches.
+ *
+ * Both: no workspace, no host synchronisation, capturable in a CUDA graph.
+ * ---------------------------------------------------------------------------------------------- */
+int sis3d_instance_paint(const uint8_t *bits, const int64_t *offs, const int32_t *box, int n_box, int x0, int y0, int z0,
+                         int X, int Y, int Z, int32_t *owner, void *stream);
+int sis3d_vertex_instance_overlap(const float *verts, int n_vert, const double *world2grid, const int32_t *owner, int x0,
+                                  int y0, int z0, int X, int Y, int Z, int canvas_x, int canvas_y, int canvas_z,
+                                  const int32_t *gt_slot, int n_slot, int n_box, int64_t *hist, int32_t *first_vertex,
+                                  int32_t *vertex_box, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
