@@ -388,6 +388,7 @@ static int linear_splits(int M, int N, int K) {
     return splits;
 }
 extern "C" size_t sis3d_linear_workspace_bytes(int M, int N, int K) {
+    if (M <= 0 || N <= 0 || K <= 0) return 0;  // linear_splits divides by the tile count
     return sizeof(float) * (size_t)linear_splits(M, N, K) * M * N + 16;
 }
 extern "C" int sis3d_linear(const float *x, const float *w_packed, const float *bias, float *y, int M, int K, int N, int act,

@@ -809,7 +809,7 @@ extern "C" int sis3d_pack_conv_weight_tc(const float *w, int cout, int cin, int 
 }
 
 extern "C" int sis3d_conv3d_k3_tc_supported(int cin, int cout) {
-    return (cin % TC_KC == 0 && (cout == 32 || cout == 64 || cout % 128 == 0)) ? 1 : 0;
+    return (cin > 0 && cout > 0 && cin % TC_KC == 0 && (cout == 32 || cout == 64 || cout % 128 == 0)) ? 1 : 0;
 }
 
 extern "C" int sis3d_pack_conv_weight_tc_x3(const float *w, int cout, int cin, int ks, float *w_x3, void *stream) {
@@ -839,7 +839,8 @@ static int conv3d_k3_tc_impl(const float *in, const float *w_tc, const float *bi
                              int res_coff, float *out, int out_ld, int out_coff, int X, int Y, int Z, int cin, int cout,
                              int ks, const int32_t *tiles, int n_tiles, int act, void *stream, int x3,
                              __half *out_split = nullptr) {
-    if (!in || !w_tc || !(out || out_split) || X <= 0 || Y <= 0 || Z <= 0 || (ks != 1 && ks != 2 && ks != 3)) return SIS3D_EINVAL;
+    if (!in || !w_tc || !(out || out_split) || X <= 0 || Y <= 0 || Z <= 0 || cin <= 0 || cout <= 0 || (ks != 1 && ks != 2 && ks != 3))
+        return SIS3D_EINVAL;
     if (out_split && (x3 != 2 || ks != 1 || cout % TC_KC || ((uintptr_t)out_split & 15))) return SIS3D_EINVAL;
     if (ks == 2 && (tiles || X < 2 || Y < 2 || Z < 2)) return SIS3D_EINVAL;
     if (x3 && tiles) return SIS3D_EUNSUPPORTED;  // the ragged mask stage does not need the compensated product
@@ -985,13 +986,13 @@ extern "C" int sis3d_conv3d_k1_tc_h3_split(const float *in, const uint16_t *w_h3
 
 // ---- bottleneck tail: 3x3x3 conv (cin -> cmid) + ReLU + 1x1 conv (cmid -> cout) + residual + act, one kernel ----------------
 extern "C" int sis3d_conv3d_k3_tc_fused_supported(int cin, int cmid, int cout) {
-    return (cin % TC_KC == 0 && ((cmid == 32 && (cout == 32 || cout == 64)) || (cmid == 64 && cout == 128))) ? 1 : 0;
+    return (cin > 0 && cin % TC_KC == 0 && ((cmid == 32 && (cout == 32 || cout == 64)) || (cmid == 64 && cout == 128))) ? 1 : 0;
 }
 static int conv3d_k3_tc_fused_impl(const float *in, const float *w2_tc, const float *bias2, const float *w3_tc,
                                    const float *bias3, const float *residual, int res_ld, int res_coff, float *out,
                                    int out_ld, int out_coff, int X, int Y, int Z, int cin, int cmid, int cout, int act,
                                    void *stream, int x3, bool presplit = false) {
-    if (!in || !w2_tc || !w3_tc || !out || X <= 0 || Y <= 0 || Z <= 0) return SIS3D_EINVAL;
+    if (!in || !w2_tc || !w3_tc || !out || X <= 0 || Y <= 0 || Z <= 0 || cin <= 0 || cmid <= 0 || cout <= 0) return SIS3D_EINVAL;
     if (presplit && x3 != 2) return SIS3D_EINVAL;
     if (!sis3d_conv3d_k3_tc_fused_supported(cin, cmid, cout)) return SIS3D_EUNSUPPORTED;
     if (((uintptr_t)in | (uintptr_t)w2_tc | (uintptr_t)w3_tc | (uintptr_t)out) & 15) return SIS3D_EINVAL;
@@ -1102,13 +1103,16 @@ static int gemm_tc_splits(int M, int N, int K, int kc) {
     int splits = max(1, min(chunks / (128 / kc), (kNumSMs + tiles - 1) / tiles));
     return splits;
 }
-extern "C" int sis3d_linear_tc_supported(int K, int N) { return (K % TC_KC == 0 && (N == 32 || N == 64 || N % 128 == 0)) ? 1 : 0; }
+extern "C" int sis3d_linear_tc_supported(int K, int N) {
+    return (K > 0 && N > 0 && K % TC_KC == 0 && (N == 32 || N == 64 || N % 128 == 0)) ? 1 : 0;
+}
 extern "C" size_t sis3d_linear_tc_workspace_bytes(int M, int N, int K) {
+    if (M <= 0 || !sis3d_linear_tc_supported(K, N)) return 0;  // gemm_tc_splits divides by the tile and chunk counts
     return sizeof(float) * (size_t)gemm_tc_splits(M, N, K, 16) * M * N + 16;  // the x3 variant splits K finer: covers both
 }
 static int linear_tc_impl(const float *x, const float *w_nk, const float *bias, float *y, int M, int K, int N, int act,
                           void *workspace, size_t workspace_bytes, void *stream, int x3) {
-    if (!x || !w_nk || !y || !workspace || M <= 0) return SIS3D_EINVAL;
+    if (!x || !w_nk || !y || !workspace || M <= 0 || K <= 0 || N <= 0) return SIS3D_EINVAL;
     if (!sis3d_linear_tc_supported(K, N)) return SIS3D_EUNSUPPORTED;
     if (((uintptr_t)x | (uintptr_t)w_nk | (uintptr_t)workspace) & 15) return SIS3D_EINVAL;
     EncodeTiledFn enc = get_encode();
@@ -1122,7 +1126,8 @@ static int linear_tc_impl(const float *x, const float *w_nk, const float *bias, 
     const int chunks = K / kc;
     const int per = cdiv(chunks, splits);
     splits = cdiv(chunks, per);
-    if (workspace_bytes < sizeof(float) * (size_t)splits * M * N) return SIS3D_EWORKSPACE;
+    // the documented size, not this mode's need: a buffer that is too small for the finest split is rejected in every mode
+    if (workspace_bytes < sis3d_linear_tc_workspace_bytes(M, N, K)) return SIS3D_EWORKSPACE;
     CUtensorMap tmA, tmB;
     {
         cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)M};
@@ -1191,7 +1196,8 @@ extern "C" int sis3d_cast_f16(const float *in, int in_ld, int in_coff, int64_t r
 extern "C" int sis3d_conv3d_tc_f16(const uint16_t *in16, const uint16_t *w16, const float *bias, const float *residual,
                                    int res_ld, int res_coff, float *out32, uint16_t *out16, int out_ld, int out_coff, int X, int Y,
                                    int Z, int cin, int cout, int ks, const int32_t *tiles, int n_tiles, int act, void *stream) {
-    if (!in16 || !w16 || (!out32 && !out16) || X <= 0 || Y <= 0 || Z <= 0 || (ks != 1 && ks != 3)) return SIS3D_EINVAL;
+    if (!in16 || !w16 || (!out32 && !out16) || X <= 0 || Y <= 0 || Z <= 0 || cin <= 0 || cout <= 0 || (ks != 1 && ks != 3))
+        return SIS3D_EINVAL;
     const int taps = ks * ks * ks;
     if (!sis3d_conv3d_k3_tc_supported(cin, cout)) return SIS3D_EUNSUPPORTED;
     if (((uintptr_t)in16 | (uintptr_t)w16 | (uintptr_t)out32 | (uintptr_t)out16) & 15) return SIS3D_EINVAL;

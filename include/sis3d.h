@@ -146,7 +146,9 @@ int sis3d_linear(const float *x, const float *w_packed, const float *bias, float
                  int act, void *workspace, size_t workspace_bytes, void *stream);
 
 /* Same layer on the tensor cores (TF32 wgmma, fp32 accumulate, split-K + deterministic reduce): w_nk is the
- * nn.Linear weight as stored, [N][K].  K % 32 == 0, N in {32, 64, 128k}. */
+ * nn.Linear weight as stored, [N][K].  K % 32 == 0, N in {32, 64, 128k}, all sizes positive (the predicate is 0 and the
+ * workspace size 0 otherwise; the call returns SIS3D_EINVAL).  workspace >= sis3d_linear_tc_workspace_bytes(M, N, K) bytes in
+ * every mode (_tc, _tc_x3, _tc_h3), SIS3D_EWORKSPACE otherwise. */
 int sis3d_linear_tc_supported(int K, int N);
 size_t sis3d_linear_tc_workspace_bytes(int M, int N, int K);
 int sis3d_linear_tc(const float *x, const float *w_nk, const float *bias, float *y, int M, int K, int N, int act,
@@ -168,7 +170,7 @@ int sis3d_mlp_tail(const float *x1, int R, int d1, const float *w2, const float 
  * sis3d_pack_conv_weight_tc ([cout][ks^3*cin]).  tiles == NULL covers the whole volume with 8x2x8 (x,y,z)
  * bricks; otherwise (brick shape from sis3d_conv3d_tc_brick) tiles int32[n_tiles][8] = {x0,y0,z0,x1,y1,z1,0,0} lists brick origins and the
  * exclusive end of the voxels to be written (ragged RoI crops packed on one canvas).
- * Requires cin % 32 == 0 and cout in {32, 64, 128k}; returns SIS3D_EUNSUPPORTED otherwise.
+ * Requires cin % 32 == 0 and cout in {32, 64, 128k}; returns SIS3D_EUNSUPPORTED otherwise (SIS3D_EINVAL for cin or cout <= 0).
  * ---------------------------------------------------------------------------------------------- */
 int sis3d_pack_conv_weight_tc(const float *w_oidhw, int cout, int cin, int ks, float *w_tc, void *stream);
 int sis3d_conv3d_k3_tc_supported(int cin, int cout);
@@ -221,7 +223,11 @@ int sis3d_linear_tc_x3(const float *x, const float *w_x3, const float *bias, flo
  * of the H100 tensor core) over 32-channel stages.  Activations stay fp32 in HBM (split in shared memory after the TMA load, |v|
  * range-limited to fp16: |v| < 65504); weights from sis3d_pack_conv_weight_tc_h3: fp16 [cout][ks^3*cin/32][64], each 128-byte
  * row = the 32 hi halves of a 32-channel K slice followed by its 32 lo halves (2*cout*ks^3*cin halves in total), so one TMA
- * row request carries both parts.  Same arguments as _x3. */
+ * row request carries both parts.  Same arguments as _x3.
+ * Accuracy: per output element |err| <= 2^-15 sqrt(sum_k (x_k w_k)^2) + 2^-22 (|bias| + |residual| + |result|), plus, where an
+ * operand lies below fp16's normal range (|v| < 2^-14: its hi part is subnormal and the split keeps its value to 2^-35 absolute),
+ * an absolute floor of 2^-34 sum_k |x_k| for weights that small (2^-34 sum_k |w_k| for activations that small).  Checked per
+ * element against fp64 by tests/test_gpu_tc_accuracy.py. */
 int sis3d_pack_conv_weight_tc_h3(const float *w_oidhw, int cout, int cin, int ks, uint16_t *w_h3, void *stream);
 int sis3d_conv3d_k3_tc_h3(const float *in, const uint16_t *w_h3, const float *bias, const float *residual,
                           int res_ld, int res_coff, float *out, int out_ld, int out_coff, int X, int Y,

@@ -108,3 +108,38 @@ def test_host_side_queries_and_argument_checks():
     assert L.sis3d_memcpy_async(None, None, C.c_size_t(16), 1, None) == -1
     assert L.sis3d_view_params_host(None, None, None, None, 1, 1, C.c_double(1), C.c_double(1), C.c_double(0), C.c_double(0), 41, 32,
                                     C.c_double(0.1), C.c_double(4.0), 8, 8, 8, None) == -1
+
+
+def test_zero_and_negative_sizes_are_rejected():
+    """cin / cout / K / N / M <= 0: the support predicates say no, the workspace queries return 0 and the entry points return
+    SIS3D_EINVAL -- before any division by the tile or chunk count (an integer division by zero kills the caller's process,
+    so the calls run in a child)."""
+    import subprocess
+    import sys
+    code = """
+import ctypes as C, sys
+sys.path[:0] = sys.argv[1:]
+from lib import _sis3d as S
+L = S.lib
+out = []
+for a, b in ((0, 32), (32, 0), (-32, 64), (64, -128), (0, 0)):
+    out += [L.sis3d_conv3d_k3_tc_supported(a, b), L.sis3d_linear_tc_supported(a, b)]
+    out += [L.sis3d_conv3d_k3_tc_fused_supported(min(a, b), 32, 32), L.sis3d_conv3d_k3_tc_fused_supported(32, a, b)]
+for m, n, k in ((0, 32, 1024), (-1, 32, 1024), (8, 0, 1024), (8, -128, 1024), (8, 32, 0), (8, 32, -32)):
+    out += [L.sis3d_linear_tc_workspace_bytes(m, n, k), L.sis3d_linear_workspace_bytes(m, n, k)]
+p = C.c_void_p(16)  # never dereferenced: the size checks come first
+for m, k, n in ((8, 0, 32), (8, 1024, 0), (0, 1024, 32), (8, -32, 32)):
+    for fn in (L.sis3d_linear_tc, L.sis3d_linear_tc_x3, L.sis3d_linear_tc_h3):
+        out.append(fn(p, p, None, p, m, k, n, 0, p, C.c_size_t(1 << 20), None) + 1)
+for cin, cout in ((0, 32), (32, 0), (-32, 32)):
+    for fn in (L.sis3d_conv3d_k3_tc_x3, L.sis3d_conv3d_k3_tc_h3):
+        out.append(fn(p, p, None, None, 0, 0, p, 32, 0, 4, 4, 4, cin, cout, 3, 1, None) + 1)
+    out.append(L.sis3d_conv3d_k3_tc(p, p, None, None, 0, 0, p, 32, 0, 4, 4, 4, cin, cout, 3, None, 0, 1, None) + 1)
+    out.append(L.sis3d_conv3d_tc_f16(p, p, None, None, 0, 0, p, None, 32, 0, 4, 4, 4, cin, cout, 3, None, 0, 1, None) + 1)
+    out.append(L.sis3d_conv3d_k3_tc_fused_h3(p, p, None, p, None, None, 0, 0, p, 32, 0, 4, 4, 4, cin, 32, cout, 1, None) + 1)
+print("nonzero", [i for i, v in enumerate(out) if v])
+"""
+    p = subprocess.run([sys.executable, "-c", code, os.path.join(ROOT, "3d-sis_b200"), ROOT], capture_output=True, text=True,
+                       timeout=120)
+    assert p.returncode == 0, f"child died (exit {p.returncode}): {p.stderr[-2000:]}"
+    assert p.stdout.split("\n")[-2] == "nonzero []", p.stdout

@@ -41,9 +41,11 @@ def conv1x1_case(S, cin, cout, dims, seed):
     return x, w, b, wh3, ys
 
 
-@pytest.mark.parametrize("cin,cout,dims", [(32, 32, (48, 24, 48)), (64, 32, (45, 27, 41)), (128, 64, (24, 12, 24))])
+@pytest.mark.parametrize("cin,cout,dims", [(32, 32, (48, 24, 48)), (64, 32, (45, 27, 41)), (128, 64, (24, 12, 24)),
+                                           (64, 256, (17, 9, 11))])
 def test_k1_split_equals_split_of_fp32_output(S, cin, cout, dims):
-    """(a) the split-pair output is split_f16x2 of the fp32 output of the same conv, bit for bit."""
+    """(a) the split-pair output is split_f16x2 of the fp32 output of the same conv, bit for bit (cout = 256: the second N
+    block writes its rows at the 2 * n0 split-row offset)."""
     x, _, b, wh3, ys = conv1x1_case(S, cin, cout, dims, cin + cout + dims[0])
     y = torch.empty(dims + (cout,), device=DEV)
     S.check(S.lib.sis3d_conv3d_k3_tc_h3(S.ptr(x), S.ptr(wh3), S.ptr(b), None, 0, 0, S.ptr(y), cout, 0, *dims, cin, cout, 1, 1,

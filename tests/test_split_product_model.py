@@ -2,7 +2,7 @@
 (3d-sis_b200/csrc/conv_tc.cu: split_f16, the X3 = 2 kernels; DESIGN.md §4.1).  v = hi + lo / 2048 with hi = fp16(v),
 lo = fp16((v - hi) * 2048); a product a*b is ah*bh + (ah*bl + al*bh) / 2048 with fp32 accumulation, the al*bl term dropped.
 The properties below are what the 'exact' mode's parity claim (integer outputs equal to the fp32 path) rests on; the kernels
-themselves are checked on the GPU (tests/test_gpu_ops.py, tests/test_gpu_forward.py)."""
+themselves are checked on the GPU (tests/test_gpu_tc_accuracy.py, tests/test_gpu_forward.py)."""
 import numpy as np
 
 
@@ -77,3 +77,54 @@ def test_dropped_low_low_term_is_below_the_operand_precision():
     bh, bl = split(b)
     dropped = np.abs(al.astype(np.float64) * bl.astype(np.float64)) / 2048 ** 2
     assert (dropped / np.abs(a.astype(np.float64) * b.astype(np.float64))).max() <= 2.0 ** -22
+
+
+def _stage_model(a, b, drop=None):
+    """The X3 = 2 main loop per output element: operands split as split_f16; each 16-element MMA summed exactly and added to
+    the stage's fresh accumulator with truncation toward zero; a stage (3 x-taps x 32 channels = 96 K-elements) folded into
+    the running sum as fmaf(cross, 2^-11, sum) (round to nearest), then its hi.hi part.  drop: "cross" (no cross terms, the
+    1x product), "albh" (one cross term), or a stage index whose cross terms are lost."""
+    def parts(v):
+        hi, lo = split(v)
+        return hi.astype(np.float64), lo.astype(np.float64)
+
+    def trunc_add(acc, t):
+        s = acc.astype(np.float64) + t
+        r = s.astype(np.float32)
+        over = np.abs(r.astype(np.float64)) > np.abs(s)
+        r[over] = np.nextafter(r[over], np.float32(0))
+        return r
+
+    (ah, al), (bh, bl) = parts(a), parts(b)
+    acc = np.zeros(a.shape[0], np.float32)
+    for st in range(a.shape[1] // 96):
+        cross = np.zeros_like(acc)
+        hh = np.zeros_like(acc)
+        for m in range(6):
+            s = slice(st * 96 + m * 16, st * 96 + m * 16 + 16)
+            if drop not in ("cross", st):
+                if drop != "albh":
+                    cross = trunc_add(cross, (al[:, s] * bh[:, s]).sum(1))
+                cross = trunc_add(cross, (ah[:, s] * bl[:, s]).sum(1))
+            hh = trunc_add(hh, (ah[:, s] * bh[:, s]).sum(1))
+        acc = (cross.astype(np.float64) * 2.0 ** -11 + acc.astype(np.float64)).astype(np.float32)
+        acc = (acc.astype(np.float64) + hh).astype(np.float32)
+    return acc
+
+
+def test_per_element_bound_separates_the_compensated_kernel_from_broken_ones():
+    """The bound of tests/test_gpu_tc_accuracy.py, |err| <= C_X3 s2 + C_T |ref| with s2 = sqrt(sum_k (x_k w_k)^2), holds for the
+    modelled kernel and is exceeded at least POWER-fold by each model of a kernel that lost (part of) the compensation, at
+    K = 27 * 32 and 27 * 256.  Keeps the GPU test's constants honest without a GPU."""
+    from test_gpu_tc_accuracy import C_T, C_X3, POWER
+    rng = np.random.default_rng(4)
+    for K in (864, 6912):
+        a = np.maximum(rng.standard_normal((2000, K)), 0).astype(np.float32)  # post-ReLU activations
+        b = (rng.standard_normal((2000, K)) / np.sqrt(K)).astype(np.float32)  # weights N(0, 1/K)
+        p = a.astype(np.float64) * b.astype(np.float64)
+        ref = p.sum(1)
+        bound = C_X3 * np.sqrt((p * p).sum(1)) + C_T * np.abs(ref)
+        ratio = lambda drop: (np.abs(_stage_model(a, b, drop).astype(np.float64) - ref) / bound).max()
+        assert ratio(None) <= 1.0, (K, ratio(None))
+        for drop in ("cross", "albh", K // 96 - 1):
+            assert ratio(drop) >= POWER, (K, drop, ratio(drop))
