@@ -36,5 +36,6 @@ template <class T> inline T atomicMin(T *p, T v) {
     while (v < old && !__atomic_compare_exchange_n(p, &old, v, true, __ATOMIC_RELAXED, __ATOMIC_RELAXED)) {}
     return old;
 }
+inline long long __double_as_longlong(double d) { long long u; std::memcpy(&u, &d, 8); return u; }
 inline double __dmul_rn(double a, double b) { volatile double r = a * b; return r; }
 inline double __dadd_rn(double a, double b) { volatile double r = a + b; return r; }

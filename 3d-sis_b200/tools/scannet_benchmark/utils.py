@@ -181,6 +181,71 @@ def read_mesh_vertices(filename):
     return out
 
 
+def read_mesh_faces(filename):
+    """The first three vertex ids of every row of the `face` element's first property, int64 [M, 3] (what the reference's
+    visualization.read_ply takes: `face[0][0..2]`, tools/visualization.py:71-72).  Quads and longer polygons give their
+    first three ids.  A file without a face element gives [0, 3].  Raises ValueError when that property is not a list,
+    when a row has fewer than three ids, or when the file ends early."""
+    if not os.path.isfile(filename):
+        raise FileNotFoundError(filename)
+    with open(filename, "rb") as f:
+        fmt, elements = _parse_ply_header(f, filename)
+        names = [e[0] for e in elements]
+        if "face" not in names:
+            return np.zeros((0, 3), np.int64)
+        at = names.index("face")
+        _, count, props = elements[at]
+        if not props or not isinstance(props[0][1], tuple):
+            raise ValueError(f"{filename}: the first property of the PLY face element is not a list")
+        if fmt == "ascii":
+            lines = f.read().decode("ascii", errors="replace").splitlines()
+            row = sum(e[1] for e in elements[:at])
+            if row + count > len(lines):
+                raise ValueError(f"{filename}: PLY data ends inside the face element")
+            out = np.zeros((count, 3), np.int64)
+            for i in range(count):
+                words = lines[row + i].split()
+                if len(words) < 4 or int(words[0]) < 3:
+                    raise ValueError(f"{filename}: PLY face {i} has fewer than three vertex ids")
+                out[i] = [int(w) for w in words[1:4]]
+            return out
+        endian = "<" if fmt == "binary_little_endian" else ">"
+        for name, n, p in elements[:at]:
+            _skip_binary_element(f, n, p, endian, filename)
+        _, ct, it = props[0][1]
+        csize = np.dtype(ct).itemsize
+        if len(props) == 1 and count > 0:  # one list per row: uniform rows (all triangles) are read as one array
+            start = f.tell()
+            head = f.read(csize)
+            if len(head) == csize:
+                k = int(np.frombuffer(head, endian + ct)[0])
+                dt = np.dtype([("n", endian + ct), ("i", endian + it, (k,))])
+                rest = f.read(count * dt.itemsize - csize)
+                if k >= 3 and len(rest) == count * dt.itemsize - csize:
+                    rows = np.frombuffer(head + rest, dt, count)
+                    if (rows["n"] == k).all():
+                        return rows["i"][:, :3].astype(np.int64)
+            f.seek(start)
+        out = np.zeros((count, 3), np.int64)
+        for i in range(count):
+            for j, (_, t) in enumerate(props):
+                if isinstance(t, tuple):
+                    b = f.read(np.dtype(t[1]).itemsize)
+                    if len(b) != np.dtype(t[1]).itemsize:
+                        raise ValueError(f"{filename}: PLY data ends inside the face element")
+                    n = int(np.frombuffer(b, endian + t[1])[0])
+                    b = f.read(n * np.dtype(t[2]).itemsize)
+                    if len(b) != n * np.dtype(t[2]).itemsize:
+                        raise ValueError(f"{filename}: PLY data ends inside the face element")
+                    if j == 0:
+                        if n < 3:
+                            raise ValueError(f"{filename}: PLY face {i} has fewer than three vertex ids")
+                        out[i] = np.frombuffer(b, endian + t[2], 3)
+                elif len(f.read(np.dtype(t).itemsize)) != np.dtype(t).itemsize:
+                    raise ValueError(f"{filename}: PLY data ends inside the face element")
+        return out
+
+
 def _read_ascii_vertices(f, elements, filename):
     lines = f.read().decode("ascii", errors="replace").splitlines()
     row = 0

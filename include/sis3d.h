@@ -411,6 +411,49 @@ int sis3d_vertex_instance_overlap(const float *verts, int n_vert, const double *
                                   const int32_t *gt_slot, int n_slot, int n_box, int64_t *hist, int32_t *first_vertex,
                                   int32_t *vertex_box, void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Result visualisation: cube meshes of label volumes and ASCII PLY text (tools/visualization.py and
+ * tools/scannet_benchmark/visualize_benchmark.py; the reference's write_mask / write_ply,
+ * tools/visualization.py:78-101, 263-324).  No allocation, no host synchronisation; every pointer is
+ * on the device.  Scans use scratch of ceil(n / SIS3D_PLY_SCAN_TILE) int64.
+ *
+ * sis3d_voxel_mesh_count: labels int32 [X][Y][Z] (C order, numpy's mask[x, y, z]).  A voxel's label is
+ * labels[i], or, when lut is not NULL, lut[labels[i]] (0 for an index outside [0, n_lut)).  A voxel is
+ * occupied when its label is > 0.  Occupied voxels are numbered in the reference's visiting order: z
+ * outermost, then y, x innermost (row r = z * Y + y).  Writes row_offsets int64 [Y*Z + 1]: the
+ * exclusive prefix of the per-row counts, row_offsets[Y*Z] = the number of occupied voxels (the one
+ * value the host reads back).  Scratch: ceil(Y*Z / SIS3D_PLY_SCAN_TILE) int64.  Four launches.
+ *
+ * sis3d_voxel_mesh: the cubes of occupied voxels k in [k0, k1) (row_offsets from the count call on the
+ * same labels; k beyond the total emits nothing), output row j = k - k0:
+ *   verts  float64 [8j .. 8j+8)[3]: make_voxel_mesh's corners from fl(c - 0.05) and fl(c + 0.95);
+ *   colors int64   [8j .. 8j+8)[3]: palette[label % 41] (palette int64 [41][3], the host's
+ *                                   int(p / 255.0 * 255), as write_ply truncates it);
+ *   faces  int64   [12j .. 12j+12)[3]: the reference's twelve triangles, vertex ids 8k + local.
+ * Any of verts / colors / faces may be NULL to skip it.  One launch.
+ *
+ * sis3d_ply_ascii_lengths / sis3d_ply_ascii: the text lines [l0, l1) of vertices then faces, line i
+ * being vertex i ("{:f} {:f} {:f} {:d} {:d} {:d}\n" of verts[i], colors[i]) for i < n_vert, else face
+ * i - n_vert ("3 {:d} {:d} {:d}\n").  '{:f}' is Python's on float64: six fractional digits correctly
+ * rounded (ties to even), "-0.000000" for negative values that round to zero, nan / inf / -inf.
+ * lengths writes offsets int64 [n + 2] (n = l1 - l0): offsets[0..n] = the exclusive prefix of the
+ * line lengths (offsets[n] = the bytes of the range) and offsets[n + 1] = the number of lines with a
+ * coordinate |v| >= 2^64, which the formatter does not handle: when it is nonzero the caller formats
+ * that range itself and does not call sis3d_ply_ascii.  The host reads offsets[n .. n+2) back.
+ * sis3d_ply_ascii writes line l0 + i at out + offsets[i].  lengths: a memset and four launches;
+ * ascii: one launch.
+ * ---------------------------------------------------------------------------------------------- */
+#define SIS3D_PLY_SCAN_TILE 2048
+int sis3d_voxel_mesh_count(const int32_t *labels, const int32_t *lut, int n_lut, int X, int Y, int Z,
+                           int64_t *row_offsets, int64_t *scratch, void *stream);
+int sis3d_voxel_mesh(const int32_t *labels, const int32_t *lut, int n_lut, int X, int Y, int Z,
+                     const int64_t *row_offsets, const int64_t *palette, int64_t k0, int64_t k1, double *verts,
+                     int64_t *colors, int64_t *faces, void *stream);
+int sis3d_ply_ascii_lengths(const double *verts, const int64_t *colors, int64_t n_vert, const int64_t *faces,
+                            int64_t n_face, int64_t l0, int64_t l1, int64_t *offsets, int64_t *scratch, void *stream);
+int sis3d_ply_ascii(const double *verts, const int64_t *colors, int64_t n_vert, const int64_t *faces, int64_t n_face,
+                    int64_t l0, int64_t l1, const int64_t *offsets, char *out, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
