@@ -231,19 +231,18 @@ extern "C" int sis3d_backproject_conv_k2s2_ex(const float *feats, float *feats_t
     a.partial = (float *)(ws + o_partial);
     a.feats_t = feats_t; a.pix = pix; a.pairs = pairs; a.n_pairs = n_pairs;
     a.C = C; a.hw = img_w * img_h; a.X = X; a.Y = Y; a.Z = Z; a.n_views = n_views; a.n0 = (int64_t)X * Y * Z;
+    // everything that can refuse the call is checked before the first launch, so a refused call writes nothing
+    const size_t smem = sizeof(float) * ((size_t)C * (SP_BM + 4) + (size_t)C * cout);
+    if (smem > 200 * 1024) return SIS3D_EUNSUPPORTED;
+    if (cudaFuncSetAttribute(cout == 64 ? (const void *)sparse_gemm_kernel<64> : (const void *)sparse_gemm_kernel<32>,
+                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+        return SIS3D_ELAUNCH;
     cudaStream_t s = (cudaStream_t)stream;
     dim3 tg(cdiv(a.hw, 32), cdiv(C, 32), n_views);
     feats_transpose_kernel2<<<tg, dim3(32, 8), 0, s>>>(feats, feats_t, C, a.hw, a.counts);
     sparse_cover_kernel<<<(int)imin64(cdiv64(a.n0, 256), kNumSMs * 8), 256, 0, s>>>(a);
-    const size_t smem = sizeof(float) * ((size_t)C * (SP_BM + 4) + (size_t)C * cout);
-    if (smem > 200 * 1024) return SIS3D_EUNSUPPORTED;
-    if (cout == 64) {
-        cudaFuncSetAttribute(sparse_gemm_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        sparse_gemm_kernel<64><<<kNumSMs * 2, 256, smem, s>>>(a, w_packed);
-    } else {
-        cudaFuncSetAttribute(sparse_gemm_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        sparse_gemm_kernel<32><<<kNumSMs * 2, 256, smem, s>>>(a, w_packed);
-    }
+    if (cout == 64) sparse_gemm_kernel<64><<<kNumSMs * 2, 256, smem, s>>>(a, w_packed);
+    else sparse_gemm_kernel<32><<<kNumSMs * 2, 256, smem, s>>>(a, w_packed);
     sparse_combine_kernel<<<(int)imin64(cdiv64((int64_t)a.n1 * (cout / 4), 256), kNumSMs * 8), 256, 0, s>>>(a, cout, out, out_ld,
                                                                                                              out_coff, (__half *)out16);
     return finish_launch(4);

@@ -11,6 +11,7 @@ import torch.nn.functional as F
 import sis3d_synth as synth
 from conftest import ROOT, load_golden
 from test_gpu_tc_accuracy import conv_accuracy, fused_accuracy, linear_accuracy
+from test_gpu_simt_accuracy import fmaf_chain_accuracy, linear_splits
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -139,13 +140,16 @@ def test_conv3d_vs_torch_fp32(S, cin, cout, ks, stride, dims, bias, res, act):
     w = (rng.standard_normal((cout, cin, ks, ks, ks)) / np.sqrt(cin * ks ** 3)).astype(np.float32)
     b = rng.standard_normal(cout).astype(np.float32) if bias else None
     pad = 1 if ks == 3 else 0
-    ref = F.conv3d(torch.from_numpy(x), torch.from_numpy(w), None if b is None else torch.from_numpy(b), stride=stride,
-                   padding=pad)
-    r = rng.standard_normal(tuple(ref.shape)).astype(np.float32) if res else None
+    xt, wt = torch.from_numpy(x).double(), torch.from_numpy(w).double()
+    acc = F.conv3d(xt, wt, stride=stride, padding=pad)[0]
+    absum = F.conv3d(xt.abs(), wt.abs(), stride=stride, padding=pad)[0]
+    r = rng.standard_normal((1,) + tuple(acc.shape)).astype(np.float32) if res else None
+    epi = torch.zeros_like(acc)
+    if bias:
+        epi = epi + torch.from_numpy(b).double()[:, None, None, None]
     if res:
-        ref = ref + torch.from_numpy(r)
-    ref = F.relu(ref) if act == 1 else (torch.sigmoid(ref) if act == 2 else ref)
-    od = tuple(ref.shape[2:])
+        epi = epi + torch.from_numpy(r[0]).double()
+    od = tuple(acc.shape[1:])
     xd = torch.from_numpy(x[0]).to(DEV).permute(1, 2, 3, 0).contiguous()  # VC
     wd = torch.from_numpy(w).to(DEV)
     ldw = (cout + 3) // 4 * 4
@@ -166,7 +170,7 @@ def test_conv3d_vs_torch_fp32(S, cin, cout, ks, stride, dims, bias, res, act):
                                    cout, ks, stride, pad, act, S.stream()))
         got = out[..., 4:].permute(3, 0, 1, 2).cpu()
         assert torch.all(out[..., :4] == 7.0)
-        torch.testing.assert_close(got, ref[0], atol=2e-5, rtol=1e-4)
+        fmaf_chain_accuracy(got, acc, absum, ks ** 3 * cin + 2, epi, act)
 
 
 def test_conv3d_regions_zero_pad_at_crop_border(S):
@@ -188,9 +192,10 @@ def test_conv3d_regions_zero_pad_at_crop_border(S):
     S.check(S.lib.sis3d_conv3d(S.ptr(sd), C.c_int64(X * Y * Z), S.ptr(packed), None, None, 0, 0, S.ptr(out), 64, 0,
                                S.ptr(regions), 2, tiles, 2, 64, 3, 1, 1, 1, S.stream()))
     for j, (c, s) in enumerate(zip(crops, sizes)):
-        ref = F.relu(F.conv3d(torch.from_numpy(scene[:, :, c[0]:c[3], c[1]:c[4], c[2]:c[5]]), torch.from_numpy(w), padding=1))[0]
+        crop, wt = torch.from_numpy(scene[:, :, c[0]:c[3], c[1]:c[4], c[2]:c[5]]).double(), torch.from_numpy(w).double()
+        acc, absum = F.conv3d(crop, wt, padding=1)[0], F.conv3d(crop.abs(), wt.abs(), padding=1)[0]
         got = out[int(offs[j]) * 64:int(offs[j + 1]) * 64].view(*s, 64).permute(3, 0, 1, 2).cpu()
-        torch.testing.assert_close(got, ref, atol=2e-5, rtol=1e-4)
+        fmaf_chain_accuracy(got, acc, absum, 54 + 2, act=1)
 
 
 @pytest.mark.parametrize("C,dims", [(64, (9, 5, 7)), (64, (48, 24, 48)), (128, (24, 12, 24)), (16, (17, 8, 3)), (8, (6, 9, 11)),
@@ -458,9 +463,10 @@ def test_linear_split_k(S, M, K, N, act):
     x = rng.standard_normal((M, K)).astype(np.float32)
     w = (rng.standard_normal((N, K)) / np.sqrt(K)).astype(np.float32)
     b = rng.standard_normal(N).astype(np.float32)
-    ref = torch.from_numpy(x) @ torch.from_numpy(w).T + torch.from_numpy(b)
-    if act:
-        ref = F.relu(ref)
+    xt, wt, bt = torch.from_numpy(x).double(), torch.from_numpy(w).double(), torch.from_numpy(b).double()
+    acc, absum = xt @ wt.T, xt.abs() @ wt.abs().T
+    splits, kps = linear_splits(M, N, K)
+    n = kps + splits + 1 if splits > 1 else K + 2
     ldw = (N + 3) // 4 * 4
     packed = torch.empty(K, ldw, device=DEV)
     wdev = torch.from_numpy(w).to(DEV).reshape(N, K, 1, 1, 1).contiguous()
@@ -474,7 +480,7 @@ def test_linear_split_k(S, M, K, N, act):
         S.check(S.lib.sis3d_linear(S.ptr(xdev), S.ptr(packed), S.ptr(bdev), S.ptr(y),
                                    M, K, N, act, S.ptr(ws), C.c_size_t(nbytes), S.stream()))
         torch.cuda.synchronize()
-        torch.testing.assert_close(y.cpu(), ref, atol=3e-5, rtol=1e-4)
+        fmaf_chain_accuracy(y.cpu(), acc, absum, n, bt.expand_as(acc), act)
 
 
 @pytest.mark.parametrize("M,K,N,act", [(200, 8192, 256, 1), (61, 1024, 128, 0), (128, 256, 64, 1), (300, 2048, 32, 1)])
@@ -555,6 +561,7 @@ def test_simt_conv_and_sparse_fp16_twin(S):
     S.check(S.lib.sis3d_conv3d_ex(S.ptr(xd), C.c_int64(X * Y * Z), S.ptr(packed), None, None, 0, 0, S.ptr(out), S.ptr(out16), cout, 0,
                                   S.ptr(regions), 1, tiles, cin, cout, 2, 2, 0, 1, S.stream()))
     torch.cuda.synchronize()
-    ref = F.relu(F.conv3d(torch.from_numpy(x), torch.from_numpy(w), stride=2))[0].permute(1, 2, 3, 0)
-    torch.testing.assert_close(out.cpu(), ref, atol=2e-5, rtol=1e-4)
+    xt, wt = torch.from_numpy(x).double(), torch.from_numpy(w).double()
+    acc, absum = F.conv3d(xt, wt, stride=2)[0].permute(1, 2, 3, 0), F.conv3d(xt.abs(), wt.abs(), stride=2)[0].permute(1, 2, 3, 0)
+    fmaf_chain_accuracy(out.cpu(), acc, absum, 8 * cin + 2, act=1)
     assert torch.equal(out16, out.half())
