@@ -9,7 +9,9 @@
 // The ScanNet benchmark's vertex transfer (sis3d_instance_paint, sis3d_vertex_instance_overlap) follows below the overlap
 // kernel: the reference paints every kept mask into a 400x200x400 float64 canvas, looks each mesh vertex up in it, writes one
 // 0/1 text line per (instance, vertex) and parses them back to count overlaps with the GT ids.  Here an int32 owner volume
-// covers only the boxes' extent, and one pass over the vertices counts vertices per (box, GT id).
+// covers only the boxes' extent, and one pass over the vertices counts vertices per (box, GT id).  The GT ids themselves can
+// come from ScanNet's segment annotations (sis3d_segment_gt_slots, at the end): a per-segment table replaces the reference's
+// per-vertex GT text files.
 #include <climits>
 #include "common.cuh"
 
@@ -160,6 +162,46 @@ vertex_overlap_kernel(const float *verts, int n_vert, const double *w2g, const i
     atomicMin(first_vertex + b, v);
 }
 
+// ------------------------------------------------------------------------------------------------------- GT from segments
+// ScanNet's annotations label segments, not vertices: the host resolves export_train_mesh_for_evaluation.py's rules once per
+// segment into a table sorted by segment id, and each vertex finds its segment's row by binary search.  Slot counts go
+// through a per-CTA shared histogram (most vertices fall into a few slots, 0 above all), flushed once per CTA.
+constexpr int kSlotThreads = 256;
+constexpr int kSlotShared = 1024;  // slots counted in shared memory; higher slots go straight to global atomics
+
+__global__ void segment_slot_init_kernel(int64_t *slot_count, int n_slot) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_slot; i += stride) slot_count[i] = 0;
+}
+
+__global__ void __launch_bounds__(kSlotThreads)
+segment_gt_slot_kernel(const int32_t *seg_index, int n_vert, const int32_t *seg_ids, const int32_t *seg_slot, int n_seg,
+                       int n_slot, int32_t *gt_slot, int64_t *slot_count) {
+    __shared__ int s_count[kSlotShared];
+    const int n_shared = min(n_slot, kSlotShared);
+    for (int i = threadIdx.x; i < n_shared; i += kSlotThreads) s_count[i] = 0;
+    __syncthreads();
+    for (int v = blockIdx.x * kSlotThreads + threadIdx.x; v < n_vert; v += gridDim.x * kSlotThreads) {
+        const int32_t seg = seg_index[v];
+        int slot = 0;
+        if (seg >= 0) {
+            int lo = 0, hi = n_seg;  // first row with seg_ids[row] >= seg
+            while (lo < hi) {
+                const int mid = (lo + hi) >> 1;
+                if (seg_ids[mid] < seg) lo = mid + 1;
+                else hi = mid;
+            }
+            if (lo < n_seg && seg_ids[lo] == seg) slot = seg_slot[lo];
+        }
+        gt_slot[v] = slot;
+        if (slot >= 0 && slot < n_shared) atomicAdd(s_count + slot, 1);
+        else if (slot >= 0 && slot < n_slot) atomicAdd((unsigned long long *)(slot_count + slot), 1ull);
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < n_shared; i += kSlotThreads)
+        if (s_count[i]) atomicAdd((unsigned long long *)(slot_count + i), (unsigned long long)s_count[i]);
+}
+
 }  // namespace sis3d
 using namespace sis3d;
 
@@ -215,6 +257,26 @@ extern "C" int sis3d_vertex_instance_overlap(const float *verts, int n_vert, con
         vertex_overlap_kernel<<<cdiv(n_vert, kVertexThreads), kVertexThreads, 0, s>>>(
             verts, n_vert, world2grid, owner, x0, y0, z0, X, Y, Z, canvas_x, canvas_y, canvas_z, gt_slot, n_slot, n_box, hist,
             first_vertex, vertex_box);
+        ++launches;
+    }
+    return launches ? finish_launch(launches) : SIS3D_OK;
+}
+
+extern "C" int sis3d_segment_gt_slots(const int32_t *seg_index, int n_vert, const int32_t *seg_ids, const int32_t *seg_slot,
+                                      int n_seg, int n_slot, int32_t *gt_slot, int64_t *slot_count, void *stream) {
+    if (n_vert < 0 || n_seg < 0 || n_slot < 0) return SIS3D_EINVAL;
+    if (n_vert > 0 && (!seg_index || !gt_slot)) return SIS3D_EINVAL;
+    if (n_seg > 0 && (!seg_ids || !seg_slot)) return SIS3D_EINVAL;
+    if (n_slot > 0 && !slot_count) return SIS3D_EINVAL;
+    cudaStream_t s = (cudaStream_t)stream;
+    int launches = 0;
+    if (n_slot > 0) {
+        segment_slot_init_kernel<<<(int)imin64(cdiv64(n_slot, 256), 4 * kNumSMs), 256, 0, s>>>(slot_count, n_slot);
+        ++launches;
+    }
+    if (n_vert > 0) {
+        segment_gt_slot_kernel<<<(int)imin64(cdiv64(n_vert, kSlotThreads), 4 * kNumSMs), kSlotThreads, 0, s>>>(
+            seg_index, n_vert, seg_ids, seg_slot, n_seg, n_slot, gt_slot, slot_count);
         ++launches;
     }
     return launches ? finish_launch(launches) : SIS3D_OK;

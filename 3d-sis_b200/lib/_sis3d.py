@@ -72,7 +72,8 @@ SYMBOLS = ["sis3d_strerror", "sis3d_version", "sis3d_launch_count", "sis3d_nms_w
            "sis3d_mask_select", "sis3d_pack_conv_weight_tc_x3", "sis3d_conv3d_k3_tc_x3", "sis3d_conv3d_k3_tc_fused_x3",
            "sis3d_linear_tc_x3", "sis3d_pack_conv_weight_tc_h3", "sis3d_conv3d_k3_tc_h3", "sis3d_conv3d_k3_tc_fused_h3",
            "sis3d_linear_tc_h3", "sis3d_chunk_decode", "sis3d_conv3d_k1_tc_h3_split", "sis3d_conv3d_k3_tc_fused_h3_split", "sis3d_mask_overlap",
-           "sis3d_instance_paint", "sis3d_vertex_instance_overlap", "sis3d_voxel_mesh_count", "sis3d_voxel_mesh",
+           "sis3d_instance_paint", "sis3d_vertex_instance_overlap", "sis3d_segment_gt_slots", "sis3d_voxel_mesh_count",
+           "sis3d_voxel_mesh",
            "sis3d_ply_ascii_lengths", "sis3d_ply_ascii"]
 # include/sis3d_enet.h
 SYMBOLS_ENET = ["sis3d_enet_pack_weight", "sis3d_enet_conv2d", "sis3d_enet_pool_affine", "sis3d_enet_to_nchw"]

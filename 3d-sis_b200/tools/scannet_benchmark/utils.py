@@ -1,11 +1,12 @@
 """File helpers of the ScanNet instance benchmark (reference: tools/scannet_benchmark/utils.py; lines cited per function).
 
-Only what the evaluator and vox2mesh's command line need: per-vertex id files, instance prediction files, GT instances, and
-the vertex positions of a PLY mesh.  The reference reads meshes with `plyfile`; `read_mesh_vertices` here parses the PLY
+Only what the evaluator, vox2mesh's command line and the GT export need: per-vertex id files, label maps, instance
+prediction files, GT instances, and the vertex positions of a PLY mesh.  The reference reads meshes with `plyfile`; `read_mesh_vertices` here parses the PLY
 header itself, so nothing beyond numpy is needed.
 """
 from __future__ import annotations
 
+import csv
 import os
 import sys
 
@@ -16,6 +17,34 @@ def print_error(message, user_fault=False):
     """utils.py:19-23: the message on stderr, then exit status 2 for a user error, -1 otherwise."""
     sys.stderr.write("ERROR: " + str(message) + "\n")
     sys.exit(2 if user_fault else -1)
+
+
+def represents_int(s):
+    """utils.py:26-31: whether int(s) succeeds."""
+    try:
+        int(s)
+        return True
+    except ValueError:
+        return False
+
+
+def read_label_mapping(filename, label_from="raw_category", label_to="nyu40id", delimiter="\t"):
+    """utils.py:33-43: `{row[label_from]: int(row[label_to])}` over the rows of a delimited file with a header row; a later
+    duplicate row wins.  When the first key represents an int, every key is converted with int()."""
+    assert os.path.isfile(filename)
+    mapping = {}
+    with open(filename) as f:
+        for row in csv.DictReader(f, delimiter=delimiter):
+            mapping[row[label_from]] = int(row[label_to])
+    if represents_int(list(mapping.keys())[0]):
+        mapping = {int(k): v for k, v in mapping.items()}
+    return mapping
+
+
+def export_ids(filename, ids):
+    """utils.py:57-60: one '%d' line per id."""
+    with open(filename, "w") as f:
+        f.write("".join("%d\n" % i for i in np.asarray(ids).tolist()))
 
 
 def load_ids(filename):

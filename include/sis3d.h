@@ -411,6 +411,20 @@ int sis3d_vertex_instance_overlap(const float *verts, int n_vert, const double *
                                   const int32_t *gt_slot, int n_slot, int n_box, int64_t *hist, int32_t *first_vertex,
                                   int32_t *vertex_box, void *stream);
 
+/* sis3d_segment_gt_slots: per-vertex GT slots from ScanNet's segment annotations (the reference's
+ * tools/scannet_benchmark/export_train_mesh_for_evaluation.py, resolved per segment on the host).
+ * Table: seg_ids int32[n_seg] sorted ascending and unique, seg_slot int32[n_seg] the slot of each
+ * segment's GT id (slot s = index of the id in the sorted distinct ids of the table with 0 added).
+ * Per vertex v: gt_slot[v] = seg_slot[row] for the row whose seg_ids equals seg_index[v]; 0 (id 0,
+ * unannotated) for a segment id not in the table or negative.  slot_count int64[n_slot] = the number
+ * of vertices per slot (slots outside [0, n_slot) are not counted); initialised by the call.  gt_slot
+ * feeds sis3d_vertex_instance_overlap directly.  SIS3D_EINVAL on a negative size or a missing
+ * pointer; n_vert = 0 only initialises slot_count.  No workspace, no host synchronisation,
+ * capturable in a CUDA graph.  Two launches.
+ * ---------------------------------------------------------------------------------------------- */
+int sis3d_segment_gt_slots(const int32_t *seg_index, int n_vert, const int32_t *seg_ids, const int32_t *seg_slot, int n_seg,
+                           int n_slot, int32_t *gt_slot, int64_t *slot_count, void *stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Result visualisation: cube meshes of label volumes and ASCII PLY text (tools/visualization.py and
  * tools/scannet_benchmark/visualize_benchmark.py; the reference's write_mask / write_ply,
