@@ -215,10 +215,11 @@ using namespace sis3d;
 extern "C" int sis3d_project_map(const float *views, const float *depth, int n_views, int img_w, int img_h,
                                  float fx, float fy, float cx, float cy, float depth_min, float depth_max, float voxel_size, int X, int Y,
                                  int Z, int16_t *pix, int32_t *counts, void *stream) {
-    if (!views || !depth || !pix || !counts || n_views <= 0 || img_w * img_h > 32767) return SIS3D_EINVAL;
+    if (!views || !depth || !pix || !counts || n_views <= 0 || img_w * img_h > 32767 || X < 0 || Y < 0 || Z < 0) return SIS3D_EINVAL;
     cudaStream_t s = (cudaStream_t)stream;
     if (cudaMemsetAsync(counts, 0, sizeof(int32_t) * n_views, s) != cudaSuccess) return SIS3D_ELAUNCH;
     const int64_t n0 = (int64_t)X * Y * Z;
+    if (n0 == 0) return SIS3D_OK;  // empty volume: every count is 0, no map entry exists
     dim3 grid((unsigned)imin64(cdiv64(n0, 256), kNumSMs * 8), n_views);
     project_map_kernel<<<grid, 256, 0, s>>>((const ViewParams *)views, depth, img_w, img_h, fx, fy, cx,
                                             cy, depth_min, depth_max, voxel_size, X, Y, Z, pix, counts);
@@ -233,9 +234,12 @@ extern "C" int sis3d_project_compact(const int16_t *pix, int X, int Y, int Z, in
                                      void *workspace, size_t workspace_bytes, void *stream) {
     const int64_t n0 = (int64_t)X * Y * Z;
     const int nblocks = (int)cdiv64(n0, kCompactBlock);
-    if (!pix || !lin3d || !lin2d || !workspace) return SIS3D_EINVAL;
+    if (!pix || !lin3d || !lin2d || !workspace || X < 0 || Y < 0 || Z < 0) return SIS3D_EINVAL;
     if (workspace_bytes < sizeof(int32_t) * (size_t)nblocks) return SIS3D_EWORKSPACE;
     cudaStream_t s = (cudaStream_t)stream;
+    if (nblocks == 0)  // empty volume: both lists hold only their count, 0
+        return cudaMemsetAsync(lin3d, 0, sizeof(int64_t), s) == cudaSuccess && cudaMemsetAsync(lin2d, 0, sizeof(int64_t), s) == cudaSuccess
+                   ? SIS3D_OK : SIS3D_ELAUNCH;
     int32_t *bc = (int32_t *)workspace;
     compact_count_kernel<<<nblocks, kCompactBlock, 0, s>>>(pix, n0, bc);
     compact_scan_kernel<<<1, 1024, 0, s>>>(bc, nblocks, lin3d, lin2d);

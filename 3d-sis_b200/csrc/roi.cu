@@ -253,6 +253,7 @@ extern "C" int sis3d_roi_pool_fwd(const float *feat, int feat_layout, float spat
                                   int height, int length, int channels, int pw, int ph, int pl, const float *rois,
                                   float *top, int32_t *argmax, void *stream) {
     if (!feat || !rois || !top || num_rois < 0 || pw <= 0 || ph <= 0 || pl <= 0 || channels <= 0) return SIS3D_EINVAL;
+    if (feat_layout != 0 && (int64_t)pw * ph > 65535) return SIS3D_EUNSUPPORTED;  // gridDim.y of the VC kernel
     if (num_rois == 0) return SIS3D_OK;
     cudaStream_t s = (cudaStream_t)stream;
     if (feat_layout == 0) {
@@ -270,7 +271,9 @@ extern "C" int sis3d_roi_pool_fwd(const float *feat, int feat_layout, float spat
 extern "C" int sis3d_roi_pool_levels(const float *feat1, const float *feat2, const float *feat3, const int32_t *level_ids,
                                      float spatial_scale, int num_rois, int width, int height, int length, int channels,
                                      int pw, int ph, int pl, const float *rois, float *top, int32_t *argmax, void *stream) {
-    if (!feat1 || !level_ids || !rois || !top || num_rois <= 0) return SIS3D_EINVAL;
+    if (!feat1 || !level_ids || !rois || !top || num_rois <= 0 || channels <= 0 || pw <= 0 || ph <= 0 || pl <= 0)
+        return SIS3D_EINVAL;
+    if ((int64_t)pw * ph > 65535) return SIS3D_EUNSUPPORTED;  // gridDim.y
     roi_pool_vc_kernel<<<dim3(num_rois, pw * ph), 128, 0, (cudaStream_t)stream>>>(feat1, feat2, feat3, level_ids, spatial_scale,
                                                                                  width, height, length, channels, pw, ph, pl,
                                                                                  rois, top, argmax);
@@ -280,7 +283,8 @@ extern "C" int sis3d_roi_pool_levels(const float *feat1, const float *feat2, con
 extern "C" int sis3d_detect_decode(const float *rois, const int32_t *num_rois, int max_rois, const float *cls_score,
                                    const float *bbox_pred, int num_classes, int scene_x, int scene_y, int scene_z,
                                    float class_thresh, float *cls_prob, int64_t *cls_pred, float *det, void *stream) {
-    if (!rois || !num_rois || !cls_score || !bbox_pred || !cls_prob || !cls_pred || !det || max_rois <= 0) return SIS3D_EINVAL;
+    if (!rois || !num_rois || !cls_score || !bbox_pred || !cls_prob || !cls_pred || !det || max_rois <= 0 || num_classes <= 0)
+        return SIS3D_EINVAL;
     detect_decode_kernel<<<cdiv(max_rois, 128), 128, 0, (cudaStream_t)stream>>>(rois, num_rois, max_rois, cls_score, bbox_pred,
                                                                               num_classes, scene_x, scene_y, scene_z,
                                                                               class_thresh, cls_prob, cls_pred, det);

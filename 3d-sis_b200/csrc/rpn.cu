@@ -313,6 +313,7 @@ __global__ void rpn_pad_kernel(float *rois, float *scores, int32_t *level_ids, c
 // Same keys (score bits | ~flat index: unique, stable descending order) and the same decode arithmetic as
 // rpn_topk_decode_kernel: identical outputs.
 constexpr int kSortCap = 4096;  // candidates sorted in shared memory (32 KB)
+constexpr size_t kReduceSmemCap = 200 * 1024;  // largest bitmask + remv words nms_reduce_smem_kernel stages (pre_top_n <= 1279)
 
 __device__ __forceinline__ void decode_box(const RpnLevels &L, int f, float *box, int &lvl_id) {
     int lvl, vox, a, x, y, z;
@@ -524,10 +525,11 @@ extern "C" int sis3d_nms(const float *boxes, int n, float thresh, int64_t *keep,
     if (n == 0) return cudaMemsetAsync(num_out, 0, sizeof(int32_t), s) == cudaSuccess ? SIS3D_OK : SIS3D_ELAUNCH;
     const int cb = cdiv(n, 64);
     if ((size_t)cb * 8 > 200 * 1024) return SIS3D_EUNSUPPORTED;
+    if ((size_t)cb * 8 > 48 * 1024 &&
+        cudaFuncSetAttribute(nms_reduce_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cb * 8) != cudaSuccess)
+        return SIS3D_ELAUNCH;
     nms_mask_kernel<<<dim3(cb, cb), 64, 0, s>>>(boxes, n, thresh, (unsigned long long *)workspace, cb);
     NmsGather g = {};
-    if ((size_t)cb * 8 > 48 * 1024)
-        cudaFuncSetAttribute(nms_reduce_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cb * 8);
     nms_reduce_kernel<<<1, 256, cb * 8, s>>>((const unsigned long long *)workspace, n, nullptr, cb, keep, num_out, g);
     return finish_launch(2);
 }
@@ -564,21 +566,37 @@ extern "C" int sis3d_rpn_proposals(const sis3d_rpn_level *lv, int n_levels, int 
     RpnWs w = carve(base, total, pre_top_n);
     if (w.bytes + 16 > workspace_bytes) return SIS3D_EWORKSPACE;
     cudaStream_t s = (cudaStream_t)stream;
+    if (total == 0) {  // every level grid is empty: no anchor, no proposal (a zero-block launch would fail)
+        const bool ok = cudaMemsetAsync(num_out, 0, sizeof(int32_t), s) == cudaSuccess &&
+                        cudaMemsetAsync(rois, 0, sizeof(float) * 6 * post_top_n, s) == cudaSuccess &&
+                        cudaMemsetAsync(scores, 0, sizeof(float) * post_top_n, s) == cudaSuccess &&
+                        cudaMemsetAsync(level_ids, 0, sizeof(int32_t) * post_top_n, s) == cudaSuccess &&
+                        (!debug_order || cudaMemsetAsync(debug_order, 0xFF, sizeof(int32_t) * pre_top_n, s) == cudaSuccess);
+        return ok ? SIS3D_OK : SIS3D_ELAUNCH;
+    }
+    const int cb = cdiv(pre_top_n, 64);
+    const size_t reduce_smem = sizeof(unsigned long long) * ((size_t)pre_top_n * cb + cb);
+    const bool fused = reduce_smem <= kReduceSmemCap && !getenv("SIS3D_RPN_UNFUSED");
+    const int Kp2 = next_pow2(pre_top_n);
+    // shared-memory opt-ins are checked before the first launch, so a refused call leaves every buffer untouched
+    if (fused) {
+        static bool attr = false;
+        if (!attr) {
+            if (cudaFuncSetAttribute(nms_reduce_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kReduceSmemCap) != cudaSuccess)
+                return SIS3D_ELAUNCH;
+            attr = true;
+        }
+    } else if ((size_t)Kp2 * 8 > 48 * 1024 &&
+               cudaFuncSetAttribute(rpn_topk_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Kp2 * 8) != cudaSuccess) {
+        return SIS3D_ELAUNCH;
+    }
     if (cudaMemsetAsync(w.hist, 0, sizeof(int) * (kHistBins + 2), s) != cudaSuccess) return SIS3D_ELAUNCH;
     const int blocks = min(cdiv(total, 256), kNumSMs * 4);
     rpn_score_kernel<<<blocks, 256, 0, s>>>(L, w.keys, w.hist);
     rpn_candidates_kernel<<<blocks, 256, 0, s>>>(w.keys, total, w.hist, pre_top_n, w.cand, w.cand_count);
-    const int cb = cdiv(pre_top_n, 64);
-    const size_t reduce_smem = sizeof(unsigned long long) * ((size_t)pre_top_n * cb + cb);
-    if (reduce_smem <= 200 * 1024 && !getenv("SIS3D_RPN_UNFUSED")) {
+    if (fused) {
         // low-latency chain: sort + decode in one CTA (candidates sorted in shared memory), the K x K/64 IoU bitmask on
         // cb x cb CTAs (the parallel part), greedy reduce + gather + padding in one CTA with the bitmask staged in shared memory
-        static bool attr = false;
-        if (!attr) {
-            if (cudaFuncSetAttribute(nms_reduce_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess)
-                return SIS3D_ELAUNCH;
-            attr = true;
-        }
         rpn_sort_decode_kernel<<<1, 1024, 0, s>>>(L, w.cand, w.cand_count, pre_top_n, w.sorted_boxes, w.sorted_scores, w.sorted_levels,
                                                 debug_order, w.n_sorted);
         nms_mask_kernel<<<dim3(cb, cb), 64, 0, s>>>(w.sorted_boxes, pre_top_n, nms_thresh, w.mask, cb);
@@ -586,9 +604,6 @@ extern "C" int sis3d_rpn_proposals(const sis3d_rpn_level *lv, int n_levels, int 
         nms_reduce_smem_kernel<<<1, 256, reduce_smem, s>>>(w.mask, pre_top_n, w.n_sorted, cb, g, num_out);
         return finish_launch(5);
     }
-    const int Kp2 = next_pow2(pre_top_n);
-    if ((size_t)Kp2 * 8 > 48 * 1024)
-        cudaFuncSetAttribute(rpn_topk_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Kp2 * 8);
     rpn_topk_decode_kernel<<<1, 1024, Kp2 * 8, s>>>(L, w.cand, w.cand_count, pre_top_n, Kp2, w.sorted_boxes, w.sorted_scores,
                                                   w.sorted_levels, debug_order, w.n_sorted);
     // NMS over the (zero padded) pre_top_n rows is wrong when fewer than pre_top_n candidates exist:

@@ -50,6 +50,8 @@ int sis3d_nms(const float *boxes, int n, float thresh, int64_t *keep, int32_t *n
  * rois [n,6]; top [n,C,pw,ph,pl]; argmax int32 same shape or NULL (indices in the NCDHW convention).
  * sis3d_roi_pool_levels is the pyramid form used by the forward (lib/nets/network.py:503-534): VC
  * features of up to three levels, level_ids int32[n] (1-based, 0 = padded row -> zeros) pick the map.
+ * channels, pw, ph and pl must be positive (SIS3D_EINVAL); the VC kernels need pw*ph <= 65535
+ * (SIS3D_EUNSUPPORTED).
  * ---------------------------------------------------------------------------------------------- */
 int sis3d_roi_pool_fwd(const float *feat, int feat_layout, float spatial_scale, int num_rois,
                        int width, int height, int length, int channels, int pw, int ph, int pl,
@@ -71,6 +73,8 @@ int sis3d_roi_pool_levels(const float *feat1, const float *feat2, const float *f
  *                         int32[n_views] = number of valid voxels per view (zeroed by the call).
  * sis3d_project_compact : ordered compaction of one view's map into the reference's (lin3d, lin2d)
  *                         int64 lists of length 1+Z*Y*X with element 0 = count.
+ * An empty volume (X*Y*Z == 0) is a defined empty result: the map call zeroes counts, the compaction
+ * writes count 0, and neither launches a kernel.  Negative extents are SIS3D_EINVAL.
  * sis3d_backproject_max : fused gather + cross-view max into a VC volume [X][Y][Z][C]; reproduces
  *                         the reference's pairing of feature maps with surviving index lists when
  *                         views are dropped (pairs from sis3d_backproject_pairs), see DESIGN.md.  feats [n_views][C][h][w]
@@ -290,6 +294,9 @@ int sis3d_vc_to_ncdhw(const float *in, float *out, int64_t nvox, int C, void *st
  * Outputs: rois [post_top_n][6], scores [post_top_n], level_ids int32[post_top_n] (1-based),
  * num_out int32[1]; debug_order int32[pre_top_n] (flat anchor index of each pre-NMS box, or NULL).
  * Tie rule: equal scores are ordered by ascending flat index (level, x, y, z, a).
+ * Rows from num_out to post_top_n are zero; debug_order rows past the candidate count are -1.  When every level
+ * grid is empty the call launches nothing and returns that empty result (num_out = 0).
+ * pre_top_n in 1..8192 and post_top_n >= 1, SIS3D_EUNSUPPORTED otherwise.
  * ---------------------------------------------------------------------------------------------- */
 typedef struct sis3d_rpn_level {
     const float *cls;
@@ -314,7 +321,8 @@ int sis3d_rpn_proposals(const sis3d_rpn_level *h_levels, int n_levels, int feat_
  * trainval.py:825-858): argmax class, softmax confidence, class-specific bbox_transform_inv,
  * clip, conf > class_thresh and round()-degenerate filter (Python-3 half-to-even).
  * det float[n][16] = pred_box(6) | conf | cls | keep | crop lo(3) hi(3) | pad   (all as float)
- * n is read from device num_rois (int32[1]) and clamped to max_rois.
+ * n is read from device num_rois (int32[1]) and clamped to max_rois.  Rows n..max_rois-1 are zero,
+ * except det[0][15], which holds n.  max_rois and num_classes must be positive (SIS3D_EINVAL).
  * ---------------------------------------------------------------------------------------------- */
 int sis3d_detect_decode(const float *rois, const int32_t *num_rois, int max_rois,
                         const float *cls_score, const float *bbox_pred, int num_classes,
