@@ -25,17 +25,18 @@ extern "C" int sis3d_mask_plan_build(const float *h_det, int n, int X, int Y, in
                                      size_t capacity, sis3d_mask_plan *plan) {
     if (!h_det || !plan || n < 0) return SIS3D_EINVAL;
     sis3d_mask_plan p = {};
-    int kept[4096];
-    for (int i = 0; i < n && p.n_kept < 4096; ++i)
-        if (h_det[i * 16 + 8] > 0.5f) kept[p.n_kept++] = i;
+    // every row with the keep flag set gets a crop (the list is as long as the detection table: no cap, no allocation)
+    for (int i = 0; i < n; ++i)
+        if (h_det[i * 16 + 8] > 0.5f) ++p.n_kept;
     const int nk = p.n_kept;
     if (nk == 0) { *plan = p; return SIS3D_OK; }
     // pass 1: sizes
     int64_t total = 0, xsum = 0;
     int ymax = 0, zmax = 0;
     int64_t ntiles = 0, t_mid = 0;
-    for (int j = 0; j < nk; ++j) {
-        const float *d = h_det + kept[j] * 16;
+    for (int i = 0; i < n; ++i) {
+        const float *d = h_det + i * 16;
+        if (!(d[8] > 0.5f)) continue;
         const int w = (int)d[12] - (int)d[9], h = (int)d[13] - (int)d[10], l = (int)d[14] - (int)d[11];
         total += (int64_t)w * h * l;
         xsum += w + 1;
@@ -67,8 +68,9 @@ extern "C" int sis3d_mask_plan_build(const float *h_det, int n, int X, int Y, in
     const int64_t cs0 = (int64_t)ymax * zmax * 64, cs1 = (int64_t)zmax * 64, cs2 = 64;
     int64_t voff = 0, xoff = 0, tile_no = 0;
     int tb = 0;
-    for (int j = 0; j < nk; ++j) {
-        const float *d = h_det + kept[j] * 16;
+    for (int i = 0, j = 0; i < n; ++i) {
+        const float *d = h_det + i * 16;
+        if (!(d[8] > 0.5f)) continue;
         const int x0 = (int)d[9], y0 = (int)d[10], z0 = (int)d[11];
         const int w = (int)d[12] - x0, h = (int)d[13] - y0, l = (int)d[14] - z0;
         const int64_t vox = (int64_t)w * h * l;
@@ -106,11 +108,12 @@ extern "C" int sis3d_mask_plan_build(const float *h_det, int n, int X, int Y, in
         last[j] = q;
         offs[j] = voff;
         cls[j] = (int32_t)d[7];
-        kidx[j] = kept[j];
+        kidx[j] = i;
         sizes[3 * j] = w; sizes[3 * j + 1] = h; sizes[3 * j + 2] = l;
         voff += vox;
         xoff += w + 1;
         tb += tl;
+        ++j;
     }
     offs[nk] = voff;
     p.tiles_first = p.tiles_last = p.tiles_mid = tb;

@@ -8,12 +8,17 @@ import pytest
 from lib import _sis3d as S
 
 
-def _plan(det, dims, ncls, use_canvas, cap=1 << 20):
-    blob = np.zeros(cap, dtype=np.uint8)
-    plan = S.MaskPlan()
-    rc = S.lib.sis3d_mask_plan_build(C.c_void_p(det.ctypes.data), det.shape[0], *dims, ncls, use_canvas,
-                                     C.c_void_p(blob.ctypes.data), C.c_size_t(cap), C.byref(plan))
-    return rc, plan, blob
+def _plan(det, dims, ncls, use_canvas, cap=1 << 20, grow=False):
+    """Run the planner; grow=True retries with the size it reports on SIS3D_EWORKSPACE (as Network._mask_branch does)."""
+    while True:
+        blob = np.zeros(cap, dtype=np.uint8)
+        plan = S.MaskPlan()
+        rc = S.lib.sis3d_mask_plan_build(C.c_void_p(det.ctypes.data), det.shape[0], *dims, ncls, use_canvas,
+                                         C.c_void_p(blob.ctypes.data), C.c_size_t(cap), C.byref(plan))
+        if rc == -3 and grow and plan.bytes > cap:
+            cap = int(plan.bytes)
+            continue
+        return rc, plan, blob
 
 
 def _dets(rng, n, dims):
@@ -27,13 +32,46 @@ def _dets(rng, n, dims):
     return det
 
 
+def _edge_dets(rng, dims):
+    """Kept crops at the edges of the brick layout: extent 1 on each axis, 1x1x1, whole 4x4x8 bricks (w, h = 0 mod 4,
+    l = 0 mod 8) and one voxel past them, at random positions."""
+    sizes = [(1, 5, 9), (6, 1, 9), (6, 5, 1), (1, 1, 1), (4, 8, 8), (8, 4, 16), (5, 9, 17), (4, 4, 8), (1, 4, 8)]
+    det = np.zeros((len(sizes), 16), dtype=np.float32)
+    for i, sz in enumerate(sizes):
+        lo = [int(rng.integers(0, d - s + 1)) for d, s in zip(dims, sz)]
+        det[i, 9:12], det[i, 12:15] = lo, [l + s for l, s in zip(lo, sz)]
+        det[i, 7], det[i, 8] = rng.integers(0, 19), 1.0
+    return det
+
+
 @pytest.mark.parametrize("seed", range(6))
 @pytest.mark.parametrize("use_canvas", [0, 1])
 def test_mask_plan_tables(seed, use_canvas):
     rng = np.random.default_rng(seed)
     dims, ncls = (45, 27, 41), 19
     det = _dets(rng, int(rng.integers(1, 40)), dims)
-    rc, p, blob = _plan(det, dims, ncls, use_canvas)
+    edges = _edge_dets(rng, dims)
+    at = int(rng.integers(0, det.shape[0] + 1))  # the edge crops sit at a random place among the others
+    _check_plan(np.ascontiguousarray(np.concatenate([det[:at], edges, det[at:]])), dims, ncls, use_canvas)
+
+
+def test_mask_plan_5000_kept_rows():
+    """More kept rows than the planner's former fixed list of 4096: every kept row gets its crop, offsets, size and bricks."""
+    rng = np.random.default_rng(11)
+    dims, n = (48, 24, 40), 5000
+    det = np.zeros((n + 300, 16), dtype=np.float32)
+    sz = rng.integers(1, 7, (n + 300, 3))
+    lo = np.stack([rng.integers(0, d - s + 1) for d, s in zip(dims, sz.T)], 1)
+    det[:, 9:12], det[:, 12:15] = lo, lo + sz
+    det[:, 7] = rng.integers(0, 19, n + 300)
+    det[rng.permutation(n + 300)[:n], 8] = 1.0   # 5000 kept rows among 5300, the last kept one near the end
+    assert int((det[:, 8] > 0.5).sum()) == n
+    for use_canvas in (0, 1):
+        _check_plan(det, dims, 19, use_canvas)
+
+
+def _check_plan(det, dims, ncls, use_canvas):
+    rc, p, blob = _plan(det, dims, ncls, use_canvas, grow=True)
     assert rc == 0
     kept = np.nonzero(det[:, 8] > 0.5)[0]
     assert p.n_kept == len(kept)
