@@ -1138,10 +1138,18 @@ class Network(nn.Module):
         self._ensure_packed()
         blobs_iter = self._reject_index_lists(blobs_iter)
         self.__dict__["_home_stream"] = torch.cuda.current_stream()  # restored after every slot switch of this loop
+        finished = False
         try:
             yield from self._scene_loop(blobs_iter)
+            finished = True
         finally:
             self.__dict__["_home_stream"] = None
+            if not finished:
+                # a consumer that stopped early (break, exception) leaves scenes in flight on their slots; the host writes
+                # those slots' pinned staging buffers (vp_host, mask tables) when it next uses them, so let the queued work end
+                for sl in self._slots:
+                    if sl["stream"] is not None:
+                        sl["stream"].synchronize()
 
     @staticmethod
     def _reject_index_lists(blobs_iter):
