@@ -7,7 +7,9 @@ mask_pred`), `_scene_info`, and `mask_backbone(scene_crop, imageft)`.
 
 Everything between the input blobs and `_predictions` runs as hand-written CUDA (csrc/*.cu) on VC
 (channels-last) activations; nn.Module is used only as the parameter container so checkpoints of the
-reference load unchanged.  Training mode is out of scope (inference-only hot path).
+reference load unchanged.  Training mode is out of scope (inference-only hot path).  With USE_RPN = USE_CLASS = False the
+forward runs on the ground-truth boxes and classes of blobs['gt_box'] (`gt_detection_table`): only the mask stage runs, and
+`_predictions` has no `level_inds` or `cls_score`, as in the reference.
 """
 from __future__ import annotations
 
@@ -95,6 +97,41 @@ class _MaskList:
 
     def __eq__(self, other):
         return list(self) == other if isinstance(other, list) else NotImplemented
+
+
+def gt_detection_table(gt_box, dims, class_thresh, num_classes):
+    """The [n, 16] detection table of ground-truth RoIs (USE_RPN = USE_CLASS = False; reference: network.py:262-265, 276-301),
+    built on the host in the layout and float32 operation order of detect_decode_kernel (csrc/roi.cu): the box decoded with
+    zero deltas and clipped to the scene, conf = 1.0 (the one-hot cls_prob at the ground-truth class), the class, the keep
+    flag (conf > CLASS_THRESH, compared in float64 as the reference's driver does, and a non-empty rounded extent on every
+    axis), the crop bounds (round half to even) and n in row 0, column 15.  gt_box: [n, >= 7] (x0, y0, z0, x1, y1, z1,
+    class)."""
+    g = np.asarray(gt_box, dtype=np.float32)
+    if g.ndim != 2 or g.shape[1] < 7:
+        raise S.Sis3dError(f"gt_box must be [n, 7] (box, class), got shape {tuple(g.shape)}")
+    if not np.isfinite(g[:, :7]).all():
+        raise S.Sis3dError("gt_box holds a non-finite value")
+    n = g.shape[0]
+    cls = np.trunc(g[:, 6]).astype(np.int64)  # gt_box[:, 6].long()
+    if n and (cls.min() < 0 or cls.max() >= num_classes):
+        raise S.Sis3dError(f"gt_box class out of range [0, {num_classes}): {cls.min()} .. {cls.max()}")
+    det = np.zeros((n, 16), dtype=np.float32)
+    lo, hi = g[:, 0:3], g[:, 3:6]
+    w = hi - lo
+    ctr = lo + np.float32(0.5) * w
+    pc = np.float32(0.0) * w + ctr                # dx * w + ctr with dx = 0
+    hw = np.float32(0.5) * (np.float32(1.0) * w)  # 0.5 * (exp(0) * w)
+    d = np.asarray(dims, dtype=np.float32)
+    det[:, 0:3] = np.minimum(np.maximum(pc - hw, np.float32(0.0)), d)
+    det[:, 3:6] = np.minimum(np.maximum(pc + hw, np.float32(0.0)), d)
+    crop = np.rint(det[:, 0:6])
+    det[:, 6] = 1.0
+    det[:, 7] = cls
+    det[:, 8] = (1.0 > float(class_thresh)) & (crop[:, 0:3] < crop[:, 3:6]).all(1)
+    det[:, 9:15] = crop
+    if n:
+        det[0, 15] = n
+    return det
 
 
 class Network(nn.Module):
@@ -969,6 +1006,16 @@ class Network(nn.Module):
             # tensors yielded by the scene loop live in slot-owned buffers (result ring, arena): whatever the consumer queued
             # on its own stream to read them (a clone, a D2H copy) must finish before this slot's stream overwrites them
             slot["stream"].wait_stream(home)
+        if not cfg.USE_RPN:
+            # ground-truth RoIs: the detection table is known on the host before any launch; nothing of the static stage
+            # (ENet, back-projection, backbone, RPN, classifier) can change an output, so none of it runs
+            if "gt_box" not in blobs:
+                raise S.Sis3dError("USE_RPN=False takes its RoIs from blobs['gt_box'], which these blobs lack")
+            gt = blobs["gt_box"][0]
+            gt = gt.cpu().numpy() if isinstance(gt, torch.Tensor) else np.asarray(gt)
+            h.update(use_graph=False, fused=None, gt_box=gt,
+                     gt_det=gt_detection_table(gt, dims, cfg.CLASS_THRESH, int(cfg.NUM_CLASSES)))
+            return h
         with torch.no_grad(), Network._UseSlot(self, slot):
             lists = cfg.USE_IMAGES and "proj_ind_3d" in blobs
             use_graph = self._use_graph and not (self._keep_debug or self._prof is not None or lists)
@@ -1055,6 +1102,9 @@ class Network(nn.Module):
                     st["ring_pos"] ^= 1
                 outs["pack"].copy_(st["outs"]["pack"], non_blocking=True)
                 scene_t = st["scene"].clone() if h["fresh"] else st["scene"]
+            elif "gt_det" in h:  # ground-truth RoIs: the scene's input copy is its only work before the mask stage
+                scene_t = data.to(dev, torch.float32, non_blocking=True).contiguous()
+                outs = None
             else:
                 scene_t = data.to(dev, torch.float32, non_blocking=True).contiguous()
                 if fused:
@@ -1077,6 +1127,8 @@ class Network(nn.Module):
 
     def _launch_ragged(self, h):
         """Step 2: wait for the detections of this scene, plan + launch its ragged mask stage, queue the readback."""
+        if "gt_det" in h:
+            return self._launch_ragged_gt(h)
         h["ev_static"].synchronize()
         outs = h["outs"]
         P = {}
@@ -1105,6 +1157,30 @@ class Network(nn.Module):
         h["P"] = P
         return h
 
+    def _launch_ragged_gt(self, h):
+        """Step 2 with ground-truth RoIs (reference: network.py:262-265, 276-317): the table was built on the host, so there
+        is nothing to wait for.  The predictions other than the masks are host tensors, as the reference's cls_pred /
+        cls_prob / bbox_pred are: the scene's only GPU work is its input copy and the mask stage."""
+        gt, det = h.pop("gt_box"), h.pop("gt_det")
+        n, nc = det.shape[0], int(cfg.NUM_CLASSES)
+        cls = torch.from_numpy(det[:, 7].astype(np.int64))
+        prob = torch.zeros(n, nc, dtype=torch.float32)
+        prob[torch.arange(n), cls] = 1.0
+        P = dict(rois=[torch.from_numpy(np.ascontiguousarray(gt[:, :6], dtype=np.float32))],
+                 roi_scores=[torch.ones(n, 1, dtype=torch.float32)], cls_pred=cls, cls_prob=prob,
+                 bbox_pred=torch.zeros(n, 6 * nc, dtype=torch.float32), detections=torch.from_numpy(det), detections_host=det)
+        with torch.no_grad(), Network._UseSlot(self, h["slot"]):
+            if cfg.USE_MASK:
+                extras = {}
+                P["mask_pred"] = [self._mask_branch(h["scene_t"], det, n, extras)]
+                if "bits_pin" in extras:
+                    h["bits_pin"] = extras.pop("bits_pin")
+                P.update(extras)
+            h["ev_done"] = torch.cuda.Event(blocking=self._blocking_sync)
+            h["ev_done"].record()
+        h["P"] = P
+        return h
+
     def _finalize(self, h):
         """Step 3: wait for the scene's last kernel / copy and hand out its predictions."""
         h["ev_done"].synchronize()
@@ -1120,8 +1196,14 @@ class Network(nn.Module):
     def _check_mode(self, mode):
         if mode != "TEST":
             raise NotImplementedError("only the inference (TEST) forward is implemented on the GPU path")
-        if not (cfg.USE_BACKBONE and cfg.USE_RPN):
-            raise NotImplementedError("USE_BACKBONE/USE_RPN=False (ground-truth RoIs) are training/ablation modes")
+        # ground-truth RoIs run with USE_RPN = USE_CLASS = False (USE_BACKBONE either way); the reference cannot run the
+        # other combinations either
+        if cfg.USE_RPN and not cfg.USE_BACKBONE:
+            raise NotImplementedError("USE_BACKBONE=False with USE_RPN=True: the RPN reads the backbone's features (the "
+                                      "reference fails with a NameError); turn USE_RPN and USE_CLASS off for ground-truth RoIs")
+        if not cfg.USE_RPN and cfg.USE_CLASS:
+            raise NotImplementedError("USE_RPN=False with USE_CLASS=True: ground-truth boxes with the classifier have no test-"
+                                      "time semantics (the reference fails with KeyError 'level_inds'); turn USE_CLASS off too")
 
     def forward(self, blobs, mode="TEST", killing_inds=None):
         """Reference-compatible synchronous forward of one scene (lib/nets/network.py:72,187-317)."""

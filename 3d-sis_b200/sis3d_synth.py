@@ -250,10 +250,12 @@ def build_case(port, c):
     return cfg, w, data, views
 
 
-def make_net(c, keep_debug=True, math="fp32", weights=None, enet=False):
+def make_net(c, keep_debug=True, math="fp32", weights=None, enet=False, gt_rois=None):
     """The product Network for a case: released yml config, seeded synthetic weights loaded through load_state_dict.
     enet=True: cfg.USE_IMAGES_GT=False -- the blobs carry RGB frames and the 2-D ENet encoder (seeded default init) is part
-    of the forward."""
+    of the forward.  gt_rois=True / False: test mode on ground-truth boxes and classes (USE_RPN = USE_CLASS = False) with
+    USE_BACKBONE on / off; the weights are those of the same model without RPN and classifier heads (the ones
+    oracle/make_golden_gt_rois.py loads into the reference)."""
     import os
     import torch
     from lib.utils.config import cfg, cfg_from_file, cfg_reset
@@ -262,11 +264,17 @@ def make_net(c, keep_debug=True, math="fp32", weights=None, enet=False):
     cfg_from_file(os.path.join(os.path.dirname(os.path.abspath(__file__)), "experiments", "cfgs", yml, "rpn_class_mask_5.yml"))
     cfg.NUM_CLASSES = 26 if c["cfgname"] == "suncg" else 19
     cfg.USE_IMAGES, cfg.USE_MASK, cfg.USE_IMAGES_GT = c["use_images"], c["use_mask"], not enet
+    if gt_rois is not None:
+        cfg.USE_RPN, cfg.USE_CLASS, cfg.USE_BACKBONE = False, False, bool(gt_rois)
     from lib.nets import backbones
     import torch as _t
     _t.manual_seed(1234)  # default-initialised tensors (the ENet encoder when enet=True) are the same in every process
     net = getattr(backbones, cfg.NET)()
     net.init_modules()
+    if weights is None and gt_rois is not None:
+        weights = {k: v for k, v in make_weights(seed=0, net=cfg.NET, use_images=c["use_images"], num_classes=cfg.NUM_CLASSES,
+                                                 a1=0, a2=0, use_mask=c["use_mask"]).items()
+                   if not k.startswith("classifier_")}
     w = weights if weights is not None else make_weights(
         seed=0, net=cfg.NET, use_images=c["use_images"], num_classes=cfg.NUM_CLASSES, a1=cfg.NUM_ANCHORS_LEVEL1,
         a2=cfg.NUM_ANCHORS_LEVEL2, use_mask=c["use_mask"])
