@@ -142,15 +142,12 @@ class Network(nn.Module):
         super().__init__()
         self._predictions = {}
         self._feat_stride = [4, 4, 4]
-        self._packed = {}
+        self._packs = {}   # form -> layer -> packed weight (pack_plan)
+        self._layers = {}  # layer -> (fp32 bias or None, cout, cin, ks)
         self._packed_version = None
         self._region_cache = {}
         self._const_cache = {}
         self._keep_debug = False
-        self._packed_tc = {}
-        self._packed_h = {}
-        self._packed_x3 = {}
-        self._packed_h3 = {}
         # conv math (see set_conv_math).  Default 'exact': error-compensated split products (fp32-class accuracy, wgmma) in the
         # static stage -- everything that decides an integer output: proposal order, NMS keep list, class argmax, crop
         # bounds -- and fp16-stored operands in the ragged mask stage, whose outputs carry the 1e-3 tolerance.
@@ -160,8 +157,6 @@ class Network(nn.Module):
         self._branches = os.environ.get("SIS3D_BRANCHES", "1") != "0"
         self._replayed_kernels = 0  # libsis3d kernels executed through CUDA-graph replays
         self._sparse_color = os.environ.get("SIS3D_SPARSE_COLOR", "1") != "0"
-        self._fuse_bneck = os.environ.get("SIS3D_FUSE_BNECK", "1") != "0"
-        self._tc_k2s2 = os.environ.get("SIS3D_TC_K2S2", "1") != "0"
         # host waits yield the core instead of spinning: with one process per GPU on a CPU-quota'd node, eight spinning
         # waiters plus the Python loops would eat the whole quota (cgroup throttling stalls every rank at once)
         # (spinning is ~9 % faster on an otherwise idle host, so it stays the default while cores are plentiful)
@@ -307,14 +302,92 @@ class Network(nn.Module):
         "fp16": ("fp16", "fp16"),
         "fp32": ("fp32", "fp32"),      # CUDA-core kernels throughout
     }
+    # A conv math names the weight form its kernels read.  Mode -> forms its static-stage convs fall back to when a layer has
+    # no pack of the mode's own form ('fp16': TF32 when no fp16 twin of the output is requested, else the CUDA-core kernel).
+    FALLBACK_FORMS = {"fp16": ("tf32",)}
+    MASK_ROUTES = ("fp32", "tf32", "fp16")  # mask-stage form -> route index of the mask stage (MaskStage.math)
+    _TC32_SUFFIX = {"tf32": "", "tf32x3": "_x3", "f16x3": "_h3"}  # tensor-core forms of the fp32-output kernels -> name suffix
+
+    @classmethod
+    def mode_forms(cls, mode):
+        """The weight forms conv math `mode` reads: the CUDA-core fp32 form, which every mode keeps (the first and last mask
+        layers, the MLP tail and the sparse colour path read it), the static-stage form, its fallbacks and the mask-stage form."""
+        static, mask = cls.MATH_MODES[mode]
+        return tuple(dict.fromkeys(("fp32", static, *cls.FALLBACK_FORMS.get(mode, ()), mask)))
+
+    @staticmethod
+    def pack_layout(form, shape):
+        """(shape, dtype) of the `form` pack of a layer whose weight has `shape` ([cout, cin, ks, ks, ks] conv or [cout, cin]
+        nn.Linear); () when the form's kernel reads the fp32 weight as it is; None when no kernel of the form takes the layer."""
+        cout, cin = shape[0], shape[1]
+        ks = shape[2] if len(shape) == 5 else 1
+        K = ks ** 3 * cin
+        if form == "fp32":  # CUDA-core kernels: [K][cout rounded up to 4]
+            return (K, (cout + 3) // 4 * 4), torch.float32
+        if len(shape) == 2:  # the tensor-core GEMM; its TF32 route reads nn.Linear's [N][K] weight, already K-major
+            if form == "fp16" or cin < 1024 or not S.lib.sis3d_linear_tc_supported(cin, cout):
+                return None
+            if form == "tf32":
+                return ()
+        elif ks not in (1, 2, 3) or not S.lib.sis3d_conv3d_k3_tc_supported(cin, cout):
+            return None
+        elif form == "fp16" and (ks == 2 or (cin % 64 and cin != 32)):  # fp16-operand kernel: no 2x2x2 taps, cin 32 or 64k
+            return None
+        rows = 2 if form in ("tf32x3", "f16x3") else 1  # the split forms keep a hi and a lo row per output channel
+        return (rows * cout, K), (torch.float16 if form in ("f16x3", "fp16") else torch.float32)
+
+    @classmethod
+    def pack_plan(cls, shapes, mode):
+        """{form: {layer: pack_layout}}: the packs `_ensure_packed` makes in conv math `mode`, from the layers' weight shapes
+        (layer -> shape): every form the mode reads, each with the layers a kernel of that form takes."""
+        return {form: {k: lay for k, s in shapes.items() if (lay := cls.pack_layout(form, s)) is not None}
+                for form in cls.mode_forms(mode)}
 
     def set_conv_math(self, mode):
         """'exact' (error-compensated fp16-split static stage + fp16-operand mask stage) | 'f16x3' | 'tf32x3' | 'mixed' (TF32 +
         fp16) | 'tf32' | 'fp16' | 'fp32' (CUDA-core path)."""
         if mode not in self.MATH_MODES:
             raise S.Sis3dError(f"unknown conv math {mode!r} ({' | '.join(self.MATH_MODES)})")
-        self.__dict__["_math"], self.__dict__["_mask_math"] = self.MATH_MODES[mode]
-        self.__dict__["_math_mode"] = mode
+        d = self.__dict__
+        old = d.get("_math_mode")
+        d["_math"], d["_mask_math"] = self.MATH_MODES[mode]
+        d["_math_mode"] = mode
+        # the static-stage forms that fp32-output tensor-core kernels read, in the order _conv tries them
+        d["_tc32_forms"] = tuple(f for f in (d["_math"], *self.FALLBACK_FORMS.get(mode, ())) if f in self._TC32_SUFFIX)
+        if old is not None and set(self.mode_forms(old)) != set(self.mode_forms(mode)):
+            d["_pack_dirty"], d["_packed_version"] = True, None  # the next forward packs the forms of this mode
+
+    def _layer_weights(self):
+        """layer -> (fp32 weight, fp32 bias or None) of every conv and linear of the 3-D model, plus per RPN level both heads
+        as ONE 1x1 conv: [2A | 6A] output channels, zero-padded to a tensor-core friendly width (32/64/128k) so the merged
+        head runs on the wgmma kernel as well."""
+        params = dict(self.named_parameters())
+        out = {}
+        for name, p in params.items():
+            if name.endswith(".weight") and not name.startswith("image_enet_"):
+                b = params.get(name[:-7] + ".bias")
+                out[name[:-7]] = (p.detach().float().contiguous(), None if b is None else b.detach().float().contiguous())
+        for lvl in (1, 2, 3):
+            c, b = out.get(f"rpn_cls_score_net_level{lvl}.0"), out.get(f"rpn_bbox_pred_net_level{lvl}")
+            if c is not None and b is not None:
+                cout = c[0].shape[0] + b[0].shape[0]
+                cpad = 32 if cout <= 32 else (64 if cout <= 64 else (cout + 127) // 128 * 128)
+                wp, bp = c[0].new_zeros(cpad, *c[0].shape[1:]), c[1].new_zeros(cpad)
+                wp[:cout], bp[:cout] = torch.cat([c[0], b[0]], 0), torch.cat([c[1], b[1]], 0)
+                out[f"rpn_heads_level{lvl}"] = (wp, bp)
+        return out
+
+    _PACKERS = {"fp32": "sis3d_pack_conv_weight", "tf32": "sis3d_pack_conv_weight_tc", "tf32x3": "sis3d_pack_conv_weight_tc_x3",
+                "f16x3": "sis3d_pack_conv_weight_tc_h3", "fp16": "sis3d_pack_conv_weight_tc_f16"}
+
+    def _pack(self, form, layer, w, layout):
+        """The `form` pack (pack_layout) of the fp32 weight `w` of `layer`."""
+        if layout == ():
+            return w
+        out = torch.empty(layout[0], dtype=layout[1], device=w.device)
+        _, cout, cin, ks = self._layers[layer]
+        S.check(getattr(S.lib, self._PACKERS[form])(S.ptr(w), cout, cin, ks, S.ptr(out), S.stream()), f"{self._PACKERS[form]}[{layer}]")
+        return out
 
     def _ensure_packed(self):
         d = self.__dict__
@@ -329,76 +402,16 @@ class Network(nn.Module):
         self._pack_dirty = False
         if v == self._packed_version:
             return
-        self._packed, self._packed_tc, self._packed_h, self._packed_x3, self._packed_h3 = {}, {}, {}, {}, {}
-        params = dict(self.named_parameters())
         self.__dict__["_enet"] = None
         if self.__dict__.get("_enet_names"):
             from lib.nets.enet import EnetEncoder
-            sd = dict(params)
+            sd = dict(self.named_parameters())
             sd.update(dict(self.named_buffers()))
             self.__dict__["_enet"] = EnetEncoder([sd[n].detach() for n in self._enet_names], d["_dev"])
-        for name, p in params.items():
-            if not name.endswith(".weight") or name.startswith("image_enet_"):
-                continue
-            base = name[:-7]
-            w = p.detach().float().contiguous()
-            if w.dim() == 2:
-                w = w.reshape(w.shape[0], w.shape[1], 1, 1, 1)
-            cout, cin, ks = w.shape[0], w.shape[1], w.shape[2]
-            ldw = (cout + 3) // 4 * 4
-            packed = torch.empty(ks ** 3 * cin, ldw, dtype=torch.float32, device=w.device)
-            S.check(S.lib.sis3d_pack_conv_weight(S.ptr(w), cout, cin, ks, S.ptr(packed), S.stream()), "pack")
-            b = params.get(base + ".bias")
-            self._packed[base] = (packed, None if b is None else b.detach().float().contiguous(), cout, cin, ks)
-            if ks in (1, 2, 3) and p.dim() == 5 and S.lib.sis3d_conv3d_k3_tc_supported(cin, cout):
-                wtc = torch.empty(cout, ks ** 3 * cin, dtype=torch.float32, device=w.device)
-                S.check(S.lib.sis3d_pack_conv_weight_tc(S.ptr(w), cout, cin, ks, S.ptr(wtc), S.stream()), "pack_tc")
-                self._packed_tc[base] = wtc
-                wx3 = torch.empty(2 * cout, ks ** 3 * cin, dtype=torch.float32, device=w.device)
-                S.check(S.lib.sis3d_pack_conv_weight_tc_x3(S.ptr(w), cout, cin, ks, S.ptr(wx3), S.stream()), "pack_x3")
-                self._packed_x3[base] = wx3
-                wh3 = torch.empty(2 * cout, ks ** 3 * cin, dtype=torch.float16, device=w.device)
-                S.check(S.lib.sis3d_pack_conv_weight_tc_h3(S.ptr(w), cout, cin, ks, S.ptr(wh3), S.stream()), "pack_h3")
-                self._packed_h3[base] = wh3
-                if ks != 2 and (cin % 64 == 0 or cin == 32):
-                    w16 = torch.empty(cout, ks ** 3 * cin, dtype=torch.float16, device=w.device)
-                    S.check(S.lib.sis3d_pack_conv_weight_tc_f16(S.ptr(w), cout, cin, ks, S.ptr(w16), S.stream()), "pack_f16")
-                    self._packed_h[base] = w16
-            elif p.dim() == 2 and cin >= 1024 and S.lib.sis3d_linear_tc_supported(cin, cout):
-                wx3 = torch.empty(2 * cout, cin, dtype=torch.float32, device=w.device)  # nn.Linear [N][K] = a 1x1 conv
-                S.check(S.lib.sis3d_pack_conv_weight_tc_x3(S.ptr(w), cout, cin, 1, S.ptr(wx3), S.stream()), "pack_x3")
-                self._packed_x3[base] = wx3
-                wh3 = torch.empty(2 * cout, cin, dtype=torch.float16, device=w.device)
-                S.check(S.lib.sis3d_pack_conv_weight_tc_h3(S.ptr(w), cout, cin, 1, S.ptr(wh3), S.stream()), "pack_h3")
-                self._packed_h3[base] = wh3
-        for lvl in (1, 2, 3):  # both RPN heads of a level as ONE 1x1 conv: [2A | 6A] output channels, zero-padded to a
-            # tensor-core friendly width (32/64/128k) so the merged head runs on the wgmma kernel as well
-            c, b = f"rpn_cls_score_net_level{lvl}.0", f"rpn_bbox_pred_net_level{lvl}"
-            if c + ".weight" in params and b + ".weight" in params:
-                w = torch.cat([params[c + ".weight"], params[b + ".weight"]], 0).detach().float()
-                bias = torch.cat([params[c + ".bias"], params[b + ".bias"]], 0).detach().float()
-                cout, cin = w.shape[0], w.shape[1]
-                cpad = 32 if cout <= 32 else (64 if cout <= 64 else (cout + 127) // 128 * 128)
-                wp = torch.zeros(cpad, cin, 1, 1, 1, dtype=torch.float32, device=w.device)
-                wp[:cout] = w
-                bp = torch.zeros(cpad, dtype=torch.float32, device=w.device)
-                bp[:cout] = bias
-                packed = torch.empty(cin, cpad, dtype=torch.float32, device=w.device)
-                S.check(S.lib.sis3d_pack_conv_weight(S.ptr(wp), cpad, cin, 1, S.ptr(packed), S.stream()), "pack")
-                self._packed[f"rpn_heads_level{lvl}"] = (packed, bp, cpad, cin, 1)
-                if S.lib.sis3d_conv3d_k3_tc_supported(cin, cpad):
-                    wtc = torch.empty(cpad, cin, dtype=torch.float32, device=w.device)
-                    S.check(S.lib.sis3d_pack_conv_weight_tc(S.ptr(wp), cpad, cin, 1, S.ptr(wtc), S.stream()), "pack_tc")
-                    self._packed_tc[f"rpn_heads_level{lvl}"] = wtc
-                    wx3 = torch.empty(2 * cpad, cin, dtype=torch.float32, device=w.device)
-                    S.check(S.lib.sis3d_pack_conv_weight_tc_x3(S.ptr(wp), cpad, cin, 1, S.ptr(wx3), S.stream()), "pack_x3")
-                    self._packed_x3[f"rpn_heads_level{lvl}"] = wx3
-                    wh3 = torch.empty(2 * cpad, cin, dtype=torch.float16, device=w.device)
-                    S.check(S.lib.sis3d_pack_conv_weight_tc_h3(S.ptr(wp), cpad, cin, 1, S.ptr(wh3), S.stream()), "pack_h3")
-                    self._packed_h3[f"rpn_heads_level{lvl}"] = wh3
-                    w16 = torch.empty(cpad, cin, dtype=torch.float16, device=w.device)
-                    S.check(S.lib.sis3d_pack_conv_weight_tc_f16(S.ptr(wp), cpad, cin, 1, S.ptr(w16), S.stream()), "pack_f16")
-                    self._packed_h[f"rpn_heads_level{lvl}"] = w16
+        weights = self._layer_weights()
+        self._layers = {k: (b, w.shape[0], w.shape[1], w.shape[2] if w.dim() == 5 else 1) for k, (w, b) in weights.items()}
+        plan = self.pack_plan({k: tuple(w.shape) for k, (w, _) in weights.items()}, self._math_mode)
+        self._packs = {form: {k: self._pack(form, k, weights[k][0], lay) for k, lay in layers.items()} for form, layers in plan.items()}
         torch.cuda.current_stream().synchronize()
         self._packed_version = v
         # captured graphs hold the addresses of the previous packed weights: drop them (re-captured on next use)
@@ -443,10 +456,12 @@ class Network(nn.Module):
 
     def _conv(self, x: Act, name, stride=1, pad=None, act=0, residual: Act = None, out: Act = None,
               regions=None, out_dims=None, want32=True, want16=False, out16=None):
-        """One convolution.  Dispatch: wgmma fp16-operand kernel ('fp16' math), wgmma TF32 kernel ('tf32'), else the
-        fp32 CUDA-core kernel.  want32/want16 choose which of the fp32 output / dense fp16 twin are produced (the twin
-        feeds the next tensor-core layer in 'fp16' math); out16 = caller-provided fp16 destination (ragged mask stage)."""
-        packed, bias, cout, cin, ks = self._packed[name]
+        """One convolution.  Dispatch: wgmma fp16-operand kernel ('fp16' math), else the fp32-output wgmma kernel of the first
+        of the mode's forms that has a pack of the layer, else the fp32 CUDA-core kernel.  want32/want16 choose which of the
+        fp32 output / dense fp16 twin are produced (the twin feeds the next tensor-core layer in 'fp16' math); out16 =
+        caller-provided fp16 destination (ragged mask stage)."""
+        bias, cout, cin, ks = self._layers[name]
+        W = self._packs
         if cin != x.C:
             raise S.Sis3dError(f"{name}: expected {cin} input channels, got {x.C}")
         if pad is None:
@@ -457,7 +472,7 @@ class Network(nn.Module):
         dev = (x.t if x.t is not None else x.h).device
         f16 = self._math == "fp16"
         if ks == 2:  # the 2x2x2 / stride-2 downsampling convs run on the tensor cores too (element-strided TMA boxes)
-            geom_ok = stride == 2 and pad == 0 and min(x.dims) >= 2 and self._tc_k2s2
+            geom_ok = stride == 2 and pad == 0 and min(x.dims) >= 2
         else:
             geom_ok = stride == 1 and pad == (1 if ks == 3 else 0)
         tc_ok = (regions_given is None and geom_ok and x.layout == "vc" and x.ld == x.C and x.coff == 0 and act in (0, 1))
@@ -472,9 +487,9 @@ class Network(nn.Module):
         h_ptr = S.ptr(out16) if out16 is not None else (S.ptr(out.h) if (want16 and twin_ok) else None)
         res_args = (S.ptr(residual.t) if residual is not None else None, residual.ld if residual is not None else 0,
                     residual.coff if residual is not None else 0)
-        if f16 and tc_ok and name in self._packed_h:
+        if f16 and tc_ok and name in W["fp16"]:
             tok = self._rec(f"conv_tc16[{name}]")
-            S.check(S.lib.sis3d_conv3d_tc_f16(S.ptr(self._half(x)), S.ptr(self._packed_h[name]), S.ptr(bias), *res_args,
+            S.check(S.lib.sis3d_conv3d_tc_f16(S.ptr(self._half(x)), S.ptr(W["fp16"][name]), S.ptr(bias), *res_args,
                                               S.ptr(out.t) if out.t is not None else None, h_ptr, out.ld, out.coff, *x.dims,
                                               cin, cout, ks, None, 0, act, S.stream()), f"conv3d_tc_f16[{name}]")
             self._rec_end(tok)
@@ -483,20 +498,14 @@ class Network(nn.Module):
             raise S.Sis3dError(f"{name}: this layer needs the fp32 activation but only the fp16 twin was produced")
         if out.t is None and h_ptr is None:
             out.t = torch.empty(*out_dims, cout, dtype=torch.float32, device=dev)
-        if self._math in ("tf32x3", "f16x3") and tc_ok and name in self._packed_x3 and out.t is not None and h_ptr is None:
-            h3 = self._math == "f16x3"
-            tok = self._rec(f"conv_tc_{'h3' if h3 else 'x3'}[{name}]")
-            fn = S.lib.sis3d_conv3d_k3_tc_h3 if h3 else S.lib.sis3d_conv3d_k3_tc_x3
-            S.check(fn(S.ptr(x.t), S.ptr((self._packed_h3 if h3 else self._packed_x3)[name]), S.ptr(bias), *res_args,
-                       S.ptr(out.t), out.ld, out.coff, *x.dims, cin, cout, ks, act, S.stream()),
-                    f"conv3d_k3_tc_x3[{name}]")
-            self._rec_end(tok)
-            return out
-        if self._math in ("tf32", "fp16") and tc_ok and name in self._packed_tc and out.t is not None and h_ptr is None:
-            tok = self._rec(f"conv_tc[{name}]")
-            S.check(S.lib.sis3d_conv3d_k3_tc(S.ptr(x.t), S.ptr(self._packed_tc[name]), S.ptr(bias), *res_args,
-                                             S.ptr(out.t), out.ld, out.coff, *x.dims, cin, cout, ks, None, 0, act, S.stream()),
-                    f"conv3d_k3_tc[{name}]")
+        # the fp32-output tensor-core kernels (out.t is set here unless an fp16 twin was requested, which they cannot write)
+        form = next((f for f in self._tc32_forms if name in W[f]), None) if tc_ok and h_ptr is None else None
+        if form is not None:
+            sfx = self._TC32_SUFFIX[form]
+            tok = self._rec(f"conv_tc{sfx}[{name}]")
+            fn = getattr(S.lib, f"sis3d_conv3d_k3_tc{sfx}")
+            S.check(fn(S.ptr(x.t), S.ptr(W[form][name]), S.ptr(bias), *res_args, S.ptr(out.t), out.ld, out.coff, *x.dims,
+                       cin, cout, ks, *((None, 0) if form == "tf32" else ()), act, S.stream()), f"conv3d_k3_tc{sfx}[{name}]")
             self._rec_end(tok)
             return out
         if regions is None:
@@ -506,7 +515,7 @@ class Network(nn.Module):
         in_sc = 1 if x.layout == "vc" else x.nvox
         xin = x.t if x.coff == 0 else x.t.reshape(-1)[x.coff:]
         tok = self._rec(f"conv[{name}]")
-        S.check(S.lib.sis3d_conv3d_ex(S.ptr(xin), C.c_int64(in_sc), S.ptr(packed), S.ptr(bias), *res_args,
+        S.check(S.lib.sis3d_conv3d_ex(S.ptr(xin), C.c_int64(in_sc), S.ptr(W["fp32"][name]), S.ptr(bias), *res_args,
                                       S.ptr(out.t) if out.t is not None else None, h_ptr, out.ld, out.coff, S.ptr(regions),
                                       regions.numel() // S.REGION_BYTES, n_tiles, cin, cout, ks, stride, pad, act, S.stream()),
                 f"conv3d[{name}]")
@@ -515,32 +524,23 @@ class Network(nn.Module):
 
     def _linear(self, x, name, act):
         """y = act(x W^T + b) through the split-K kernel (classifier MLP + heads)."""
-        packed, bias, cout, cin, _ = self._packed[name]
+        bias, cout, cin, _ = self._layers[name]
         M = x.shape[0]
         y = torch.empty(M, cout, dtype=torch.float32, device=x.device)
-        if self._math in ("tf32x3", "f16x3") and name in self._packed_x3:
-            h3 = self._math == "f16x3"
+        sfx = self._TC32_SUFFIX.get(self._math)
+        w = self._packs[self._math].get(name) if sfx is not None else None
+        if w is not None:
             nbytes = int(S.lib.sis3d_linear_tc_workspace_bytes(M, cout, cin))
             ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
-            tok = self._rec(f"linear_tc_{'h3' if h3 else 'x3'}[{name}]")
-            fn = S.lib.sis3d_linear_tc_h3 if h3 else S.lib.sis3d_linear_tc_x3
-            S.check(fn(S.ptr(x), S.ptr((self._packed_h3 if h3 else self._packed_x3)[name]), S.ptr(bias), S.ptr(y), M, cin, cout, act,
-                       S.ptr(ws), C.c_size_t(nbytes), S.stream()), f"linear_tc_x3[{name}]")
-            self._rec_end(tok)
-            return y
-        if self._math == "tf32" and cin >= 1024 and S.lib.sis3d_linear_tc_supported(cin, cout):
-            w_nk = dict(self.named_parameters())[name + ".weight"].detach()  # nn.Linear layout [N][K] is already K-major
-            nbytes = int(S.lib.sis3d_linear_tc_workspace_bytes(M, cout, cin))
-            ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
-            tok = self._rec(f"linear_tc[{name}]")
-            S.check(S.lib.sis3d_linear_tc(S.ptr(x), S.ptr(w_nk), S.ptr(bias), S.ptr(y), M, cin, cout, act, S.ptr(ws),
-                                          C.c_size_t(nbytes), S.stream()), f"linear_tc[{name}]")
+            tok = self._rec(f"linear_tc{sfx}[{name}]")
+            S.check(getattr(S.lib, f"sis3d_linear_tc{sfx}")(S.ptr(x), S.ptr(w), S.ptr(bias), S.ptr(y), M, cin, cout, act,
+                                                            S.ptr(ws), C.c_size_t(nbytes), S.stream()), f"linear_tc{sfx}[{name}]")
             self._rec_end(tok)
             return y
         nbytes = int(S.lib.sis3d_linear_workspace_bytes(M, cout, cin))
         ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
         tok = self._rec(f"linear[{name}]")
-        S.check(S.lib.sis3d_linear(S.ptr(x), S.ptr(packed), S.ptr(bias), S.ptr(y), M, cin, cout, act, S.ptr(ws),
+        S.check(S.lib.sis3d_linear(S.ptr(x), S.ptr(self._packs["fp32"][name]), S.ptr(bias), S.ptr(y), M, cin, cout, act, S.ptr(ws),
                                    C.c_size_t(nbytes), S.stream()), f"linear[{name}]")
         self._rec_end(tok)
         return y
@@ -550,14 +550,13 @@ class Network(nn.Module):
         activations exist only as fp16 (they feed tensor-core layers only); the block output is fp32 (+ fp16 twin when it
         is a dense tensor, for the next block's first conv)."""
         n1, n2, n3 = name + ".conv1", name + ".conv2", name + ".conv3"
-        x3 = self._math in ("tf32x3", "f16x3")
-        h3 = self._math == "f16x3"
-        wt = self._packed_h3 if h3 else (self._packed_x3 if x3 else self._packed_tc)
-        if (h3 and self._fuse_bneck and n1 in wt and n2 in wt and n3 in wt and x.t is not None and x.layout == "vc"
+        L, wt = self._layers, self._packs[self._math]
+        sfx = self._TC32_SUFFIX.get(self._math)  # the fused conv2 + conv3 kernels take the fp32-output tensor-core forms
+        if (self._math == "f16x3" and n1 in wt and n2 in wt and n3 in wt and x.t is not None and x.layout == "vc"
                 and x.ld == x.C and x.coff == 0):
-            _, b1, c1, cin1, ks1 = self._packed[n1]
-            _, _, cmid, cin, _ = self._packed[n2]
-            cout = self._packed[n3][2]
+            b1, c1, cin1, ks1 = L[n1]
+            _, cmid, cin, _ = L[n2]
+            cout = L[n3][1]
             if ks1 == 1 and cin1 == x.C and c1 == cin and S.lib.sis3d_conv3d_k3_tc_fused_supported(cin, cmid, cout):
                 # conv1 writes its activation already split into fp16 hi / lo pairs, the form the tail's MMAs read: the tail
                 # needs no operand split on the SM (the result bits are those of the fp32 hand-off below)
@@ -570,25 +569,23 @@ class Network(nn.Module):
                     out = Act(torch.empty(*x.dims, cout, dtype=torch.float32, device=x.t.device), x.dims, cout)
                 tok = self._rec(f"conv_tc_fused_h3_split[{name}]")
                 S.check(S.lib.sis3d_conv3d_k3_tc_fused_h3_split(
-                    S.ptr(ys), S.ptr(wt[n2]), S.ptr(self._packed[n2][1]), S.ptr(wt[n3]), S.ptr(self._packed[n3][1]), S.ptr(x.t),
+                    S.ptr(ys), S.ptr(wt[n2]), S.ptr(L[n2][0]), S.ptr(wt[n3]), S.ptr(L[n3][0]), S.ptr(x.t),
                     x.ld, x.coff, S.ptr(out.t), out.ld, out.coff, *x.dims, cin, cmid, cout, 1, S.stream()),
                     f"conv3d_k3_tc_fused_h3_split[{name}]")
                 self._rec_end(tok)
                 return out
         y = self._conv(x, n1, act=1, want32=False, want16=True)
-        if self._math in ("tf32", "tf32x3", "f16x3") and self._fuse_bneck and n2 in wt and n3 in wt and y.t is not None:
-            _, _, cmid, cin, _ = self._packed[n2]
-            cout = self._packed[n3][2]
+        if sfx is not None and n2 in wt and n3 in wt and y.t is not None:
+            _, cmid, cin, _ = L[n2]
+            cout = L[n3][1]
             if y.ld == y.C and y.coff == 0 and S.lib.sis3d_conv3d_k3_tc_fused_supported(cin, cmid, cout):
                 # conv2 + conv3 (+x, ReLU) in one wgmma kernel: the cmid-wide activation never leaves the SM
                 if out is None:
                     out = Act(torch.empty(*y.dims, cout, dtype=torch.float32, device=y.t.device), y.dims, cout)
-                tok = self._rec(f"conv_tc_fused{'_h3' if h3 else '_x3' if x3 else ''}[{name}]")
-                fn = (S.lib.sis3d_conv3d_k3_tc_fused_h3 if h3 else S.lib.sis3d_conv3d_k3_tc_fused_x3 if x3
-                      else S.lib.sis3d_conv3d_k3_tc_fused)
-                S.check(fn(S.ptr(y.t), S.ptr(wt[n2]), S.ptr(self._packed[n2][1]),
-                           S.ptr(wt[n3]), S.ptr(self._packed[n3][1]), S.ptr(x.t), x.ld, x.coff, S.ptr(out.t), out.ld, out.coff, *y.dims, cin,
-                           cmid, cout, 1, S.stream()), f"conv3d_k3_tc_fused[{name}]")
+                tok = self._rec(f"conv_tc_fused{sfx}[{name}]")
+                S.check(getattr(S.lib, f"sis3d_conv3d_k3_tc_fused{sfx}")(
+                    S.ptr(y.t), S.ptr(wt[n2]), S.ptr(L[n2][0]), S.ptr(wt[n3]), S.ptr(L[n3][0]), S.ptr(x.t), x.ld, x.coff,
+                    S.ptr(out.t), out.ld, out.coff, *y.dims, cin, cmid, cout, 1, S.stream()), f"conv3d_k3_tc_fused{sfx}[{name}]")
                 self._rec_end(tok)
                 return out
         y = self._conv(y, n2, act=1, want32=False, want16=True)
@@ -673,7 +670,7 @@ class Network(nn.Module):
         if (self._sparse_color and not self._keep_debug and first[0] == "k2s2" and feats.shape[1] % 16 == 0
                 and first[3] in (32, 64)):
             # fused + sparse: never materialise the back-projected volume (csrc/sparse.cu)
-            packed, _, cout, cin, _ = self._packed[f"color.{first[1]}"]
+            packed, cout = self._packs["fp32"][f"color.{first[1]}"], self._layers[f"color.{first[1]}"][1]
             od = tuple(d // 2 for d in dims)
             out = Act(torch.empty(*od, cout, dtype=torch.float32, device=dev), od, cout)
             if self._math == "fp16":
@@ -803,12 +800,11 @@ class Network(nn.Module):
         else:
             cls_t = torch.empty(R, nc, dtype=torch.float32, device=dev)
             box_t = torch.empty(R, nc * 6, dtype=torch.float32, device=dev)
-        p2, p3 = self._packed["classifier.2"], self._packed["classifier.4"]
-        pc, pb = self._packed["classifier_cls_score_net"], self._packed["classifier_bbox_pred_net"]
+        W, L = self._packs["fp32"], self._layers
+        tail = [a for k in ("classifier.2", "classifier.4", "classifier_cls_score_net", "classifier_bbox_pred_net")
+                for a in (S.ptr(W[k]), S.ptr(L[k][0]), L[k][1])]  # CUDA-core pack, bias, cout of each layer
         tok = self._rec("mlp_tail")
-        S.check(S.lib.sis3d_mlp_tail(S.ptr(x1), R, p2[3], S.ptr(p2[0]), S.ptr(p2[1]), p2[2], S.ptr(p3[0]), S.ptr(p3[1]), p3[2],
-                                     S.ptr(pc[0]), S.ptr(pc[1]), pc[2], S.ptr(pb[0]), S.ptr(pb[1]), pb[2], S.ptr(cls_t),
-                                     S.ptr(box_t), S.stream()), "mlp_tail")
+        S.check(S.lib.sis3d_mlp_tail(S.ptr(x1), R, L["classifier.2"][2], *tail, S.ptr(cls_t), S.ptr(box_t), S.stream()), "mlp_tail")
         self._rec_end(tok)
         cls_score, bbox_pred = Act(cls_t, (R, 1, 1), nc), Act(box_t, (R, 1, 1), nc * 6)
         if self._keep_debug:
@@ -824,14 +820,15 @@ class Network(nn.Module):
         and travel in ONE pinned H2D copy; all buffers come from a grow-only arena."""
         dev = scene_ncdhw.device
         X, Y, Z = (int(v) for v in scene_ncdhw.shape[2:])
-        ncls = self._packed["mask_backbone.geometry.10"][2]
-        use_tc = self._mask_math in ("tf32", "fp16") and "mask_backbone.geometry.2" in self._packed_tc
+        ncls = self._layers["mask_backbone.geometry.10"][1]
+        math = self.MASK_ROUTES.index(self._mask_math)  # route: 0 CUDA-core, 1 TF32, 2 fp16 operands (the 64->64 layers)
+        W = self._packs
         det_host = np.ascontiguousarray(det_host[:n], dtype=np.float32)
         plan = S.MaskPlan()
         cap = self._arena["mask_tables_host"].numel() if "mask_tables_host" in self._arena else 1 << 18
         while True:
             stage = self._ws("mask_tables_host", cap, torch.uint8, dev, pinned=True)
-            rc = S.lib.sis3d_mask_plan_build(C.c_void_p(det_host.ctypes.data), n, X, Y, Z, ncls, 1 if use_tc else 0,
+            rc = S.lib.sis3d_mask_plan_build(C.c_void_p(det_host.ctypes.data), n, X, Y, Z, ncls, 1 if math else 0,
                                              C.c_void_p(stage.data_ptr()), C.c_size_t(stage.numel()), C.byref(plan))
             if rc == -3:  # SIS3D_EWORKSPACE: grow the pinned staging buffer and retry
                 cap = int(plan.bytes) * 2
@@ -845,16 +842,13 @@ class Network(nn.Module):
         host = stage.numpy()
         offs = host[plan.off_offs:plan.off_offs + 8 * (nk + 1)].view(np.int64).copy()
         sizes = host[plan.off_sizes:plan.off_sizes + 12 * nk].view(np.int32).reshape(nk, 3).copy()
-        math = 0 if not use_tc else (2 if (self._mask_math == "fp16" and "mask_backbone.geometry.2" in self._packed_h) else 1)
         cvox = int(plan.canvas[0]) * int(plan.canvas[1]) * int(plan.canvas[2])
         a = S.MaskStage()
         a.scene, a.X, a.Y, a.Z, a.ncls, a.math = scene_ncdhw.data_ptr(), X, Y, Z, ncls, math
-        a.w_first = self._packed["mask_backbone.geometry.0"][0].data_ptr()
-        a.w_last = self._packed["mask_backbone.geometry.10"][0].data_ptr()
-        table = (self._packed, self._packed_tc, self._packed_h)[math]
+        a.w_first = W["fp32"]["mask_backbone.geometry.0"].data_ptr()
+        a.w_last = W["fp32"]["mask_backbone.geometry.10"].data_ptr()
         for i, idx in enumerate((2, 4, 6, 8)):
-            w = table[f"mask_backbone.geometry.{idx}"]
-            a.w_mid[i] = (w[0] if math == 0 else w).data_ptr()
+            a.w_mid[i] = W[self._mask_math][f"mask_backbone.geometry.{idx}"].data_ptr()
         a.tables = self._ws("mask_tables", nbytes, torch.uint8, dev).data_ptr()
         a.canvas_bytes = 2 * 64 * (total * 4 if math == 0 else cvox * (2 if math == 2 else 4))
         a.canvas = self._ws("mask_canvas", a.canvas_bytes, torch.uint8, dev).data_ptr()
