@@ -16,6 +16,7 @@ from __future__ import annotations
 import ctypes as C
 import gc
 import math
+import operator
 import os
 import weakref
 
@@ -28,6 +29,9 @@ from lib.layer_utils import projection as proj
 from lib.layer_utils.generate_anchors import read_anchor_sizes
 from lib.layer_utils.proposal_layer import rpn_proposals
 from lib.utils.config import cfg
+
+
+_VERSION = operator.attrgetter("_version")  # in-place update counter of a tensor
 
 
 class Act:
@@ -287,9 +291,16 @@ class Network(nn.Module):
             self._arena[name] = t
         return t[:numel]
 
+    def _versioned(self):
+        """The tensors the packed weights are made from: every parameter, and the 2-D encoder's buffers."""
+        ts = [p for _, p in self.named_parameters()]
+        if self.__dict__.get("_enet_names"):  # BatchNorm statistics of the 2-D encoder are buffers
+            ts += [b for _, b in self.named_buffers()]
+        return ts
+
     def _version(self):
         v = tuple((n, p._version, p.data_ptr()) for n, p in self.named_parameters())
-        if self.__dict__.get("_enet_names"):  # BatchNorm statistics of the 2-D encoder are buffers
+        if self.__dict__.get("_enet_names"):
             v += tuple((n, b._version, b.data_ptr()) for n, b in self.named_buffers())
         return v
 
@@ -392,7 +403,10 @@ class Network(nn.Module):
     def _ensure_packed(self):
         d = self.__dict__
         if not d["_pack_dirty"] and d["_packed_version"] is not None:  # per-scene fast path: no module traversal
-            return
+            # a parameter updated in place (p.mul_(), p.copy_(), an optimizer step) bumps its version counter and must be
+            # repacked; inside the scene loop (scenes in flight on the slots) the check runs once, when the loop starts
+            if d.get("_home_stream") is not None or list(map(_VERSION, d["_packed_from"])) == d["_packed_versions"]:
+                return
         if not torch.cuda.is_available():
             raise S.Sis3dError("the sm_90a hot path needs a CUDA device (no CPU fallback)")
         if next(self.parameters()).device.type != "cuda":
@@ -400,6 +414,8 @@ class Network(nn.Module):
         d["_dev"] = next(self.parameters()).device
         v = self._version()
         self._pack_dirty = False
+        d["_packed_from"] = self._versioned()
+        d["_packed_versions"] = list(map(_VERSION, d["_packed_from"]))
         if v == self._packed_version:
             return
         self.__dict__["_enet"] = None

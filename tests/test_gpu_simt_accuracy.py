@@ -111,19 +111,25 @@ def _raw(t):
     return t.view({torch.float32: torch.int32, torch.float16: torch.int16}.get(t.dtype, t.dtype))
 
 
-def fmaf_chain_accuracy(got, acc, absum, n, epi=None, act=0):
+def fmaf_chain_accuracy(got, acc, absum, n, epi=None, act=0, mutants=None, what="fmaf chain"):
     """Assert got == act(acc + epi) within the bound of an fmaf chain of depth n, per element: gamma_n (absum + |epi|), a
-    quarter of it + 2^-21 through a sigmoid (act = 2).  acc / absum: fp64 sum_k x_k w_k / sum_k |x_k w_k|.  Returns max err / bound."""
+    quarter of it + 2^-21 through a sigmoid (act = 2).  acc / absum: fp64 sum_k x_k w_k / sum_k |x_k w_k|.  Returns max err / bound.
+    mutants: optional fp64 models (name -> pre-activation output) that must each miss the bound by POWER somewhere; with
+    them, returns (max err / bound, smallest model max err / bound)."""
     epi = torch.zeros_like(acc) if epi is None else epi
     bound = gamma(n) * (absum + epi.abs())
     ref = acc + epi
+    f = (lambda v: v)
     if act == 2:
-        ref, bound = torch.sigmoid(ref), bound / 4 + SIG_FLOOR
+        f, bound = torch.sigmoid, bound / 4 + SIG_FLOOR
     elif act == 1:
-        ref = F.relu(ref)
+        f = F.relu
+    if mutants is not None:
+        return _check(got, f(ref), bound, {k: f(v) for k, v in mutants.items()}, 0, what)
+    ref = f(ref)
     e = (got.double().to(ref.device) - ref).abs()
     k = torch.where(e == 0, torch.zeros_like(e), e / bound).max().item()
-    assert k <= 1.0, f"max err/bound {k:.3g}"
+    assert k <= 1.0, f"{what}: max err/bound {k:.3g}"
     return k
 
 

@@ -36,6 +36,7 @@ C_X3 = 2.0 ** -15     # compensated products: 22-bit operands, short fresh accum
 C_1X = 2.0 ** -7      # one TF32 (operands truncated to 11 bits by the tensor core) or fp16 (rounded) product
 C_T = 2.0 ** -22      # fp32 roundings of the epilogue (bias, residual, output) relative to |bias| + |residual| + |ref|
 C_FLOOR = 2.0 ** -34  # fp16 split of an operand below 2^-14 (subnormal hi): 2^-35 absolute (tests/test_split_product_model.py)
+C_H = 2.0 ** -11      # rounding of an output stored as fp16 only, relative to |ref|
 POWER = 4.0           # every broken-kernel model exceeds the bound by this factor somewhere in the case
 COMPENSATED = ("x3", "h3", "h3s")
 X3_OF = {"tf32": 0, "f16": 0, "x3": 1, "h3": 2, "h3s": 2}
@@ -178,29 +179,33 @@ def _gemm(x, w):
     return x @ w.T
 
 
-def _drop_mask(mode, w):
+def _drop_mask(mode, w, slice_=None):
     """Weights whose products a broken-kernel model loses: the centre x-tap (compensated, ks 3 / 2; every output voxel has
-    it), else the last 32-channel K slice (of the centre tap for the 1x modes)."""
+    it), else one 32-channel K slice (of the centre tap for the 1x modes): slice `slice_` when given, else the last.  Real
+    activations can leave a slice all zero (dead ReLU channels); their callers pick the slice with the most input energy."""
     m = torch.zeros_like(w)
+    ks = slice(-32, None) if slice_ is None else slice(32 * slice_, 32 * slice_ + 32)
     if w.dim() == 2 or w.shape[2] == 1:
-        m[:, -32:] = 1
+        m[:, ks] = 1
     elif mode in COMPENSATED:
         m[:, :, w.shape[2] // 2] = 1
     else:
         c = w.shape[2] // 2
-        m[:, -32:, c, c, c] = 1
+        m[:, ks, c, c, c] = 1
     return m
 
 
-def _product(mode, lin, x, w):
+def _product(mode, lin, x, w, slice_=None, models=True):
     """fp64 accumulator of the linear operator lin(x, w), its error bound c * s2 (+ the subnormal floor of the fp16 split),
-    and the accumulators of the broken-kernel models."""
+    and the accumulators of the broken-kernel models (none when models is False; slice_: see _drop_mask)."""
     acc = lin(x, w)
     bound = (C_X3 if mode in COMPENSATED else C_1X) * lin(x * x, w * w).sqrt()
     if mode in ("h3", "h3s"):
         small = lambda v: (v.abs() < 2.0 ** -14).double()
         bound = bound + C_FLOOR * (lin(x.abs(), small(w)) + lin(small(x), w.abs()))
-    m = _drop_mask(mode, w)
+    if not models:
+        return acc, bound, {}
+    m = _drop_mask(mode, w, slice_)
     if mode in COMPENSATED:
         xh, wh = hi_part(x, mode), hi_part(w, mode)
         mutants = {"uncompensated": lin(xh, wh), "one_tap_no_cross": acc - lin(x, w * m) + lin(xh, wh * m)}
@@ -211,7 +216,7 @@ def _product(mode, lin, x, w):
 
 def _check(got, ref, bound, mutants, act, what):
     """Assert |got - ref| <= bound everywhere and that every broken-kernel model exceeds it by POWER somewhere.
-    Returns (kernel's max err / bound, smallest model max err / bound)."""
+    Returns (kernel's max err / bound, smallest model max err / bound; inf without models)."""
     f = F.relu if act == 1 else (lambda v: v)
     ref = f(ref)
 
@@ -223,19 +228,27 @@ def _check(got, ref, bound, mutants, act, what):
     m = {name: ratio(f(v)) for name, v in mutants.items()}
     msg = f"{what}: kernel max err/bound {k:.3g}; broken-kernel models " + ", ".join(f"{n} {v:.3g}" for n, v in m.items())
     assert k <= 1.0, msg
-    assert min(m.values()) >= POWER, "bound too loose to reject a broken kernel: " + msg
-    return k, min(m.values())
+    assert not m or min(m.values()) >= POWER, "bound too loose to reject a broken kernel: " + msg
+    return k, min(m.values(), default=math.inf)
+
+
+def _models(extra, ref):
+    """Extra fp64 models of a caller (name -> pre-activation output, or a function of the pre-activation reference)."""
+    return {k: v(ref) if callable(v) else v for k, v in (extra or {}).items()}
 
 
 def _d(t):
     return None if t is None else t.to(DEV).double()
 
 
-def conv_accuracy(mode, got, x, w, b=None, r=None, act=1, where=None, what="conv"):
+def conv_accuracy(mode, got, x, w, b=None, r=None, act=1, where=None, what="conv", slice_=None, models=True, extra=None,
+                  out16=False):
     """got: VC output [Xo][Yo][Zo][cout] of the conv of VC x [X][Y][Z][cin] with w [cout][cin][k][k][k] (+ b, + r, ReLU if
-    act == 1) in math mode `mode`; where: optional bool [Xo][Yo][Zo] of the voxels to compare."""
+    act == 1) in math mode `mode`; where: optional bool [Xo][Yo][Zo] of the voxels to compare.  models: whether the
+    broken-kernel models must miss the bound; extra: further models (_models); out16: got was stored as fp16 (adds its
+    rounding, 2^-11 |ref|, and 2^-25 below fp16's normal range)."""
     ks = w.shape[2]
-    acc, bound, mut = _product(mode, lambda a, v: _conv(a, v, ks), _d(x), _d(w))
+    acc, bound, mut = _product(mode, lambda a, v: _conv(a, v, ks), _d(x), _d(w), slice_, models)
     epi = torch.zeros_like(acc)
     if b is not None:
         epi = epi + _d(b)
@@ -243,7 +256,10 @@ def conv_accuracy(mode, got, x, w, b=None, r=None, act=1, where=None, what="conv
         epi = epi + _d(r)
     ref = acc + epi
     bound = bound + C_T * ((_d(b).abs() if b is not None else 0) + (_d(r).abs() if r is not None else 0) + ref.abs())
+    if out16:
+        bound = bound + C_H * ref.abs() + 2.0 ** -25
     mut = {k: v + epi for k, v in mut.items()}
+    mut.update(_models(extra, ref))
     got = got.to(DEV)
     if where is not None:
         where = where.to(DEV)
@@ -251,33 +267,40 @@ def conv_accuracy(mode, got, x, w, b=None, r=None, act=1, where=None, what="conv
     return _check(got, ref, bound, mut, act, what)
 
 
-def fused_accuracy(mode, got, x, w2, b2, w3, b3, r=None, act=1, what="fused"):
-    """conv2 (3x3x3, + b2) -> ReLU -> conv3 (1x1, + b3) -> + r -> act; conv2's bound propagates through |w3|."""
+def fused_accuracy(mode, got, x, w2, b2, w3, b3, r=None, act=1, what="fused", bound_in=None, slice_=None, models=True,
+                   extra=None):
+    """conv2 (3x3x3, + b2) -> ReLU -> conv3 (1x1, + b3) -> + r -> act; conv2's bound propagates through |w3|.  bound_in:
+    optional per-element error bound of x itself (a conv1 output the kernel computed), carried through w2 in quadrature."""
     lin3, lin1 = (lambda a, v: _conv(a, v, 3)), (lambda a, v: _conv(a, v, 1))
-    acc2, bound2, mut2 = _product(mode, lin3, _d(x), _d(w2))
+    acc2, bound2, mut2 = _product(mode, lin3, _d(x), _d(w2), slice_, models)
+    if bound_in is not None:
+        bound2 = bound2 + lin3(_d(bound_in) ** 2, _d(w2) ** 2).sqrt()
     b2, w3, b3 = _d(b2), _d(w3), _d(b3)
     y_pre = acc2 + b2
     y = F.relu(y_pre)
     if mode in ("h3", "h3s"):
         assert y.abs().max().item() < 65504, "inputs violate the fp16 split's range precondition"
     bound_y = bound2 + C_T * (b2.abs() + y_pre.abs())
-    acc3, bound3, _ = _product(mode, lin1, y, w3)
+    acc3, bound3, _ = _product(mode, lin1, y, w3, models=False)
     epi = b3 + (_d(r) if r is not None else 0)
     ref = acc3 + epi
     # the cmid channels' errors are independent roundings, so they add in quadrature through w3 like the products in s2; a sum
     # of |w3| bound_y is sqrt(cmid) looser and cannot reject a tail whose 3x3x3 conv lost its compensation
     bound = bound3 + lin1(bound_y ** 2, w3 ** 2).sqrt() + C_T * (b3.abs() + (_d(r).abs() if r is not None else 0) + ref.abs())
     mut = {k: lin1(F.relu(v + b2), w3) + epi for k, v in mut2.items()}
+    mut.update(_models(extra, ref))
     return _check(got.to(DEV), ref, bound, mut, act, what)
 
 
-def linear_accuracy(mode, got, x, w, b=None, act=1, what="linear"):
+def linear_accuracy(mode, got, x, w, b=None, act=1, what="linear", slice_=None, models=True, extra=None):
     """got [M][N] = act(x [M][K] . w [N][K]^T + b)."""
-    acc, bound, mut = _product(mode, _gemm, _d(x), _d(w))
+    acc, bound, mut = _product(mode, _gemm, _d(x), _d(w), slice_, models)
     epi = _d(b) if b is not None else torch.zeros_like(acc)
     ref = acc + epi
     bound = bound + C_T * (epi.abs() + ref.abs())
-    return _check(got.to(DEV), ref, bound, {k: v + epi for k, v in mut.items()}, act, what)
+    mut = {k: v + epi for k, v in mut.items()}
+    mut.update(_models(extra, ref))
+    return _check(got.to(DEV), ref, bound, mut, act, what)
 
 
 # ------------------------------------------------------------------------------------------------ inputs and launches
