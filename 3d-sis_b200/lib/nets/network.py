@@ -1040,7 +1040,12 @@ class Network(nn.Module):
             if use_graph:
                 nv = fused["feats"].shape[0] if fused else 0
                 fc = tuple(fused["feats"].shape[1:]) if fused else ()
-                key = (dims, nv, fc, self._math)
+                # the head's test-time settings are kernel arguments and buffer sizes of the captured graph: a changed
+                # pre / post-NMS count, NMS or class threshold must not replay a graph captured with the old ones
+                t = cfg.TEST
+                head = (int(t.RPN_PRE_NMS_TOP_N), int(t.RPN_POST_NMS_TOP_N), float(t.RPN_NMS_THRESH), float(cfg.CLASS_THRESH),
+                        int(cfg.ALLOW_BORDER))
+                key = (dims, nv, fc, self._math, head)
                 seen = self._shape_seen[key] = self._shape_seen.get(key, 0) + 1
                 if seen < self._graph_after and key not in self._graphs:
                     use_graph = h["use_graph"] = False  # first sight of this shape: run eagerly, capture when it comes back

@@ -508,20 +508,26 @@ class RpnEmptyCase:
         return {}
 
 
-def check_order_margin(got_flat, flat_inside, p64, K):
+def check_order_margin(got_flat, flat_inside, p64, K, either_set=False, stats=None):
     """The pre-NMS order policy for softmax scores (module docstring): got_flat must equal the fp64 order (ties by flat index)
     except for permutations among neighbours closer than twice the 12u p score bound; fails if the K-th boundary lies in that
-    band.  Returns the smallest neighbour gap outside the band."""
+    band, unless `either_set`: then the top K may take any members of the near-tied run that straddles the boundary.
+    `stats` (a dict) receives the number of near-tied neighbour pairs among the top K (`order_in_band`) and whether the
+    boundary was one of them (`boundary_in_band`).  Returns the smallest neighbour gap outside the band."""
     sb = 12 * U * p64
     srt = flat_inside[np.lexsort((flat_inside, -p64[flat_inside]))]
     gap = -np.diff(p64[srt])
     band = gap <= 2 * (sb[srt][:-1] + sb[srt][1:])
-    if K < len(srt):
-        assert not band[K - 1], "the top-K boundary lies inside the expf band: reseed this case"
-    cid = np.concatenate([[0], np.cumsum(~band)])[:K]
-    pos = {f: i for i, f in enumerate(srt[:K])}
+    at_edge = K < len(srt) and bool(band[K - 1])
+    if stats is not None:
+        stats.update(order_in_band=int(band[:K].sum()), boundary_in_band=at_edge)
+    if not either_set:
+        assert not at_edge, "the top-K boundary lies inside the expf band: reseed this case"
+    cid = np.concatenate([[0], np.cumsum(~band)])
+    pos = {f: i for i, f in enumerate(srt if at_edge else srt[:K])}
     assert all(f in pos for f in got_flat), "the top-K set differs outside the near-tie band"
-    assert np.array_equal(np.array([cid[pos[f]] for f in got_flat]), cid), "the order differs outside the near-tie band"
+    assert len(set(got_flat.tolist())) == len(got_flat), "the top K repeat an anchor"
+    assert np.array_equal(np.array([cid[pos[f]] for f in got_flat]), cid[:K]), "the order differs outside the near-tie band"
     return float(gap[:K][~band[:K]].min()) if (~band[:K]).any() else math.inf
 
 

@@ -435,6 +435,28 @@ def mlp(R, d1, d2, d3, nc, nb, *, graph=False, emu=True):
                 emu=emu, kernels=["mlp_tail_kernel"])
 
 
+def mlp_forward(x, layers, drop=None):
+    """fp64 forward of mlp_tail (two ReLU layers, then the class and box heads on the second one's output) from input x and
+    layers [(w [N][K], b [N])] x 4, with the fmaf-chain bound carried through the layers.  drop = (layer, k0): that layer's
+    weight columns k0..k0+31 zeroed (a broken kernel that skips one 32-row slab).  Returns the flattened [class | box]
+    outputs and their bounds."""
+    h = x.to(DEV).double()
+    e = torch.zeros_like(h)
+    outs_, bounds = [], []
+    for i, (w, b) in enumerate(layers):
+        w, b = w.to(DEV).double().clone(), b.to(DEV).double()
+        if drop is not None and drop[0] == i:
+            w[:, drop[1]:drop[1] + 32] = 0
+        pre = h @ w.T + b
+        eb = e @ w.abs().T + gamma(w.shape[1] + 1) * ((h.abs() + e) @ w.abs().T + b.abs())
+        if i < 2:
+            h, e = F.relu(pre), eb
+        else:
+            outs_.append(pre)
+            bounds.append(eb.expand_as(pre))
+    return torch.cat([v.reshape(-1) for v in outs_]), torch.cat([v.reshape(-1) for v in bounds])
+
+
 class MlpCase:
     def __init__(self, row):
         g = _gen(row)
@@ -474,24 +496,7 @@ class MlpCase:
         """fp64 forward with the bound carried through the layers; broken models drop one 32-row slab of one layer."""
         r = self.row
         L = [(w.to(DEV).double(), b.to(DEV).double()) for w, b in self.layers]
-
-        def forward(drop=None):
-            h = self.x.to(DEV).double()
-            e = torch.zeros_like(h)
-            outs_, bounds = [], []
-            for i, (w, b) in enumerate(L):
-                w = w.clone()
-                if drop is not None and drop[0] == i:
-                    w[:, drop[1]:drop[1] + 32] = 0
-                pre = h @ w.T + b
-                eb = e @ w.abs().T + gamma(w.shape[1] + 1) * ((h.abs() + e) @ w.abs().T + b.abs())
-                if i < 2:
-                    h, e = F.relu(pre), eb
-                else:
-                    outs_.append(pre)
-                    bounds.append(eb.expand_as(pre))
-            return torch.cat([v.reshape(-1) for v in outs_]), torch.cat([v.reshape(-1) for v in bounds])
-
+        forward = lambda drop=None: mlp_forward(self.x, L, drop)
         ref, bound = forward()
         d1, d2, d3 = r["d"]
         mut = {"layer2_slab0": forward((0, 0))[0], "layer3_last_slab": forward((1, (d2 - 1) // 32 * 32))[0],

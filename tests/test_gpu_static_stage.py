@@ -59,10 +59,10 @@ ROUTE_CHECKS = {
 OUT_OF_SCOPE = {
     "project_map": "tests/test_gpu_decision_kernels.py",
     "backproject_max": "tests/test_gpu_decision_kernels.py, tests/test_gpu_forward.py (bit exact to the oracle)",
-    "rpn_proposals": "tests/test_gpu_decision_kernels.py",
-    "roi_pool_levels": "tests/test_gpu_decision_kernels.py",
-    "mlp_tail": "tests/test_gpu_simt_accuracy.py",
-    "detect_decode": "tests/test_gpu_decision_kernels.py",
+    "rpn_proposals": "tests/test_gpu_head_stage.py, tests/test_gpu_decision_kernels.py",
+    "roi_pool_levels": "tests/test_gpu_head_stage.py, tests/test_gpu_decision_kernels.py",
+    "mlp_tail": "tests/test_gpu_head_stage.py, tests/test_gpu_simt_accuracy.py",
+    "detect_decode": "tests/test_gpu_head_stage.py, tests/test_gpu_decision_kernels.py",
     "mask_stage": "tests/test_gpu_mask_stage.py",
     "enet_encoder": "tests/test_gpu_enet.py",
 }
@@ -137,7 +137,8 @@ class Capture:
     """Wraps the static stage's op methods on one Network instance and records every call (see the module docstring)."""
     HOOKED = ("_conv", "_bottleneck", "_linear", "_pool", "_backproject")
 
-    def __init__(self, net):
+    def __init__(self, net, hooked=HOOKED):
+        self.hooked = tuple(hooked)
         self.net, self.ops, self.stack, self.loose, self.mute = net, [], [], [], False
         rec = net._rec
 
@@ -147,11 +148,11 @@ class Capture:
             return rec(name)
 
         net.__dict__["_rec"] = on_rec
-        for fn in self.HOOKED:
+        for fn in self.hooked:
             net.__dict__[fn] = self._wrap(fn[1:], getattr(net, fn))
 
     def detach(self):
-        for fn in self.HOOKED + ("_rec",):
+        for fn in self.hooked + ("_rec",):
             self.net.__dict__.pop(fn, None)
 
     def _wrap(self, kind, orig):
