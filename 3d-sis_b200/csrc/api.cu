@@ -19,8 +19,9 @@ extern "C" int64_t sis3d_launch_count(void) { return (int64_t)sis3d::g_launch_co
 // ---- host-side planner of the ragged mask stage (pure CPU code: the "runtime" part of the per-RoI mask head) ------
 // From the decoded detection table it lays out, in one byte blob that the caller ships with a single pinned H2D copy:
 // region tables of the first (windowed NCDHW scene -> canvas/compact) and last (-> dense per-crop output) layers, the
-// 4x4x8 brick list of the tensor-core layers (canvas mode) or the region table of the middle layers (compact mode), voxel
-// offsets, predicted classes, kept row indices and crop sizes.  Mirrors lib/nets/network.py:296-311 (crop selection).
+// brick list of the tensor-core layers (canvas mode; 4x4x8 bricks, from sis3d_conv3d_tc_brick) or the region table of the
+// middle layers (compact mode), voxel offsets, predicted classes, kept row indices and crop sizes.  Mirrors
+// lib/nets/network.py:296-311 (crop selection).
 extern "C" int sis3d_mask_plan_build(const float *h_det, int n, int X, int Y, int Z, int ncls, int use_canvas, void *h_blob,
                                      size_t capacity, sis3d_mask_plan *plan) {
     if (!h_det || !plan || n < 0) return SIS3D_EINVAL;
@@ -34,6 +35,8 @@ extern "C" int sis3d_mask_plan_build(const float *h_det, int n, int X, int Y, in
     int64_t total = 0, xsum = 0;
     int ymax = 0, zmax = 0;
     int64_t ntiles = 0, t_mid = 0;
+    int32_t brick[3];  // the bricks of the tensor-core layers' tile lists
+    sis3d_conv3d_tc_brick(1, 3, 64, 64, &brick[0], &brick[1], &brick[2]);
     for (int i = 0; i < n; ++i) {
         const float *d = h_det + i * 16;
         if (!(d[8] > 0.5f)) continue;
@@ -42,7 +45,7 @@ extern "C" int sis3d_mask_plan_build(const float *h_det, int n, int X, int Y, in
         xsum += w + 1;
         ymax = h > ymax ? h : ymax;
         zmax = l > zmax ? l : zmax;
-        ntiles += (int64_t)((w + 3) / 4) * ((h + 3) / 4) * ((l + 7) / 8);  // 4x4x8 bricks (sis3d_conv3d_tc_brick, tile-list mode)
+        ntiles += (int64_t)((w + brick[0] - 1) / brick[0]) * ((h + brick[1] - 1) / brick[1]) * ((l + brick[2] - 1) / brick[2]);
         t_mid += ((int64_t)w * h * l + SIS3D_CONV_TILE_M - 1) / SIS3D_CONV_TILE_M;
     }
     p.total_voxels = total;
@@ -88,9 +91,9 @@ extern "C" int sis3d_mask_plan_build(const float *h_det, int n, int X, int Y, in
             f.out_stride[0] = cs0; f.out_stride[1] = cs1; f.out_stride[2] = cs2;
             q.in_off = xoff * cs0;
             q.in_stride[0] = cs0; q.in_stride[1] = cs1; q.in_stride[2] = cs2;
-            for (int bx = 0; bx < w; bx += 4)
-                for (int by = 0; by < h; by += 4)
-                    for (int bz = 0; bz < l; bz += 8) {
+            for (int bx = 0; bx < w; bx += brick[0])
+                for (int by = 0; by < h; by += brick[1])
+                    for (int bz = 0; bz < l; bz += brick[2]) {
                         int32_t *t = tiles + tile_no * 8;
                         t[0] = (int32_t)xoff + bx; t[1] = by; t[2] = bz;
                         t[3] = (int32_t)xoff + w; t[4] = h; t[5] = l; t[6] = t[7] = 0;

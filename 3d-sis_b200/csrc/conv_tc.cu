@@ -22,6 +22,7 @@
 // rpn_net_level{1,2} (lib/nets/network.py:40,45), MaskBackbone.geometry.{2,4,6,8} (backbones.py:243-249).
 #include <cuda.h>
 #include <stdlib.h>
+#include <string.h>
 #include <cuda_fp16.h>
 #include "common.cuh"
 
@@ -743,33 +744,39 @@ static EncodeTiledFn get_encode() {
     return fn;
 }
 
-template <int BN, int KS, int EB = 4, int ROWB = 128, int BY = 2, int N2 = 0, int X3 = 0, int CL = 1, bool PS = false>
-static int launch_tc(const CUtensorMap &tmA, const CUtensorMap &tmB, const TcArgs &a_in, int n_tiles, cudaStream_t s,
-                     const CUtensorMap *tmB2 = nullptr, int grid_z = 1) {
+// template arguments of one conv3d_k3_tc_kernel instance
+struct TcInst {
+    int bn, ks, eb, rowb, by, n2, x3, cl, ps;
+    bool operator==(const TcInst &o) const { return memcmp(this, &o, sizeof o) == 0; }
+};
+
+// Launches this instance if t holds its template arguments, and sets rc to the launch's return code; false otherwise.
+template <int BN, int KS, int EB, int ROWB, int BY, int N2, int X3, int CL, bool PS>
+static bool launch_tc(const TcInst &t, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmB2, const TcArgs &a,
+                      cudaStream_t s, int grid_z, int &rc) {
+    if (!(t == TcInst{BN, KS, EB, ROWB, BY, N2, X3, CL, PS})) return false;
     const size_t smem = tc_smem_bytes<BN, KS, ROWB, BY, N2, X3>();
     auto kern = conv3d_k3_tc_kernel<BN, KS, EB, ROWB, BY, N2, X3, CL, PS>;
     static bool attr_done = false;
+    rc = SIS3D_ELAUNCH;
     if (!attr_done) {
-        if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-            return SIS3D_ELAUNCH;
+        if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return true;
         attr_done = true;
     }
-    TcArgs a = a_in;
-    a.n_tiles = n_tiles;
-    const int threads = TC_THREADS;
-    dim3 grid((n_tiles + CL - 1) / CL * CL, N2 > 0 ? 1 : a.cout / BN, grid_z);
+    dim3 grid((a.n_tiles + CL - 1) / CL * CL, N2 > 0 ? 1 : a.cout / BN, grid_z);
     if constexpr (CL == 1) {
-        kern<<<grid, threads, smem, s>>>(tmA, tmB, tmB2 ? *tmB2 : tmB, a);
+        kern<<<grid, TC_THREADS, smem, s>>>(tmA, tmB, tmB2, a);
     } else {  // thread-block cluster of CL CTAs along x (pairs of bricks)
         cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = grid; cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem; cfg.stream = s;
+        cfg.gridDim = grid; cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = s;
         cudaLaunchAttribute at[1];
         at[0].id = cudaLaunchAttributeClusterDimension;
         at[0].val.clusterDim.x = CL; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
         cfg.attrs = at; cfg.numAttrs = 1;
-        if (cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmB2 ? *tmB2 : tmB, a) != cudaSuccess) return SIS3D_ELAUNCH;
+        if (cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmB2, a) != cudaSuccess) return true;
     }
-    return finish_launch();
+    rc = finish_launch();
+    return true;
 }
 
 // fp32 [cout][cin][taps] -> fp16 [cout][taps*cin] (k = tap*cin + c), round to nearest even
@@ -828,358 +835,6 @@ extern "C" int sis3d_pack_conv_weight_tc_h3(const float *w, int cout, int cin, i
     return finish_launch();
 }
 
-// SIS3D_CLUSTER=1 turns the 2-CTA weight-tile multicast ON (off by default: multicast halves the weight bytes each SM
-// fetches, but not the rate at which an SM receives TMA rows; kept as an A/B switch)
-static bool use_cluster() {
-    static const bool on = getenv("SIS3D_CLUSTER") != nullptr && getenv("SIS3D_CLUSTER")[0] == '1';
-    return on;
-}
-
-static int conv3d_k3_tc_impl(const float *in, const float *w_tc, const float *bias, const float *residual, int res_ld,
-                             int res_coff, float *out, int out_ld, int out_coff, int X, int Y, int Z, int cin, int cout,
-                             int ks, const int32_t *tiles, int n_tiles, int act, void *stream, int x3,
-                             __half *out_split = nullptr) {
-    if (!in || !w_tc || !(out || out_split) || X <= 0 || Y <= 0 || Z <= 0 || cin <= 0 || cout <= 0 || (ks != 1 && ks != 2 && ks != 3))
-        return SIS3D_EINVAL;
-    if (out_split && (x3 != 2 || ks != 1 || cout % TC_KC || ((uintptr_t)out_split & 15))) return SIS3D_EINVAL;
-    if (ks == 2 && (tiles || X < 2 || Y < 2 || Z < 2)) return SIS3D_EINVAL;
-    if (x3 && tiles) return SIS3D_EUNSUPPORTED;  // the ragged mask stage does not need the compensated product
-    const int taps = ks * ks * ks;
-    // explicit tile lists (ragged RoI crops) use 4x4x8 bricks, whole volumes 8x2x8 (sis3d_conv3d_tc_brick)
-    const int by = (tiles && ks == 3 && cout == 64 && cin % 64 == 0) ? 4 : 2, bx = 16 / by;
-    if (!sis3d_conv3d_k3_tc_supported(cin, cout)) return SIS3D_EUNSUPPORTED;
-    if (((uintptr_t)in | (uintptr_t)w_tc | (uintptr_t)out) & 15) return SIS3D_EINVAL;
-    if ((out_ld | out_coff | res_ld | res_coff) & 3) return SIS3D_EINVAL;
-    EncodeTiledFn enc = get_encode();
-    if (!enc) return SIS3D_EUNSUPPORTED;
-    const int BN = cout >= 128 ? 128 : cout;
-    // x3 = 1 (TF32 split): 64-byte K rows (SWIZZLE_64B) so hi + lo tiles fit the same smem; x3 = 2 (fp16 split): 128-byte fp32
-    // activation rows, pre-split fp16 weights in 64-byte rows
-    const int kc = x3 == 1 ? 16 : TC_KC;
-    const CUtensorMapSwizzle sw = x3 == 1 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
-    const CUtensorMapSwizzle swb = x3 == 1 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
-    const CUtensorMapDataType dtb = x3 == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
-    const cuuint64_t wb = x3 == 2 ? 2 : 4;  // weight element bytes
-    const int sd = ks == 2 ? 2 : 1;                   // ks == 2 is the stride-2, pad-0 conv: X, Y, Z are the INPUT extents
-    const int Xo = X / sd, Yo = Y / sd, Zo = Z / sd;  // output extents (floor, as nn.Conv3d)
-    CUtensorMap tmA, tmB;
-    {
-        cuuint64_t dims[4] = {(cuuint64_t)cin, (cuuint64_t)Z, (cuuint64_t)Y, (cuuint64_t)X};
-        cuuint64_t strides[3] = {(cuuint64_t)cin * 4, (cuuint64_t)Z * cin * 4, (cuuint64_t)Y * Z * cin * 4};
-        // with element strides the box is given in traversed elements: N loaded voxels = boxDim / stride
-        cuuint32_t box[4] = {(cuuint32_t)kc, (cuuint32_t)(TC_BZ * sd), (cuuint32_t)(by * sd), (cuuint32_t)((ks == 3 ? bx + 2 : bx) * sd)};
-        cuuint32_t estr[4] = {1, (cuuint32_t)sd, (cuuint32_t)sd, (cuuint32_t)sd};
-        if (enc(&tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void *)in, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-            return SIS3D_EINVAL;
-    }
-    {
-        // x3 = 1: hi rows, then lo rows; x3 = 2: [32 hi | 32 lo] halves per 32-channel K slice in one 128-byte row
-        cuuint64_t dims[2] = {(cuuint64_t)taps * cin * (x3 == 2 ? 2 : 1), (cuuint64_t)cout * (x3 == 1 ? 2 : 1)};
-        cuuint64_t strides[1] = {dims[0] * wb};
-        cuuint32_t box[2] = {(cuuint32_t)(x3 == 2 ? 64 : kc), (cuuint32_t)BN};
-        cuuint32_t estr[2] = {1, 1};
-        if (enc(&tmB, dtb, 2, (void *)w_tc, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                swb, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-            return SIS3D_EINVAL;
-    }
-    TcArgs a;
-    a.bias = bias; a.res = residual; a.out = out; a.tiles = tiles; a.out16 = nullptr; a.bias_mid = nullptr; a.out_split = out_split;
-    a.X = Xo; a.Y = Yo; a.Z = Zo; a.cin = cin; a.cout = cout; a.act = act;
-    a.out_ld = out_ld; a.out_coff = out_coff; a.res_ld = res_ld; a.res_coff = res_coff;
-    a.tiles_y = cdiv(Yo, by); a.tiles_z = cdiv(Zo, TC_BZ);
-    if (!tiles) n_tiles = cdiv(Xo, bx) * a.tiles_y * a.tiles_z;
-    if (n_tiles <= 0) return SIS3D_OK;
-    cudaStream_t s = (cudaStream_t)stream;
-    if (x3 == 2) {
-        if (ks == 3) {
-            switch (BN) {
-                case 32: return launch_tc<32, 3, 4, 128, 2, 0, 2>(tmA, tmB, a, n_tiles, s);
-                case 64: return launch_tc<64, 3, 4, 128, 2, 0, 2>(tmA, tmB, a, n_tiles, s);
-                default: return use_cluster() ? launch_tc<128, 3, 4, 128, 2, 0, 2, 2>(tmA, tmB, a, n_tiles, s)
-                                              : launch_tc<128, 3, 4, 128, 2, 0, 2>(tmA, tmB, a, n_tiles, s);
-            }
-        }
-        if (ks == 2) {
-            switch (BN) {
-                case 32: return launch_tc<32, 2, 4, 128, 2, 0, 2>(tmA, tmB, a, n_tiles, s);
-                case 64: return launch_tc<64, 2, 4, 128, 2, 0, 2>(tmA, tmB, a, n_tiles, s);
-                default: return launch_tc<128, 2, 4, 128, 2, 0, 2>(tmA, tmB, a, n_tiles, s);
-            }
-        }
-        switch (BN) {
-            case 32: return launch_tc<32, 1, 4, 128, 2, 0, 2>(tmA, tmB, a, n_tiles, s);
-            case 64: return launch_tc<64, 1, 4, 128, 2, 0, 2>(tmA, tmB, a, n_tiles, s);
-            default: return launch_tc<128, 1, 4, 128, 2, 0, 2>(tmA, tmB, a, n_tiles, s);
-        }
-    }
-    if (x3) {
-        if (ks == 3) {
-            switch (BN) {
-                case 32: return launch_tc<32, 3, 4, 64, 2, 0, 1>(tmA, tmB, a, n_tiles, s);
-                case 64: return launch_tc<64, 3, 4, 64, 2, 0, 1>(tmA, tmB, a, n_tiles, s);
-                default: return launch_tc<128, 3, 4, 64, 2, 0, 1>(tmA, tmB, a, n_tiles, s);
-            }
-        }
-        if (ks == 2) {
-            switch (BN) {
-                case 32: return launch_tc<32, 2, 4, 64, 2, 0, 1>(tmA, tmB, a, n_tiles, s);
-                case 64: return launch_tc<64, 2, 4, 64, 2, 0, 1>(tmA, tmB, a, n_tiles, s);
-                default: return launch_tc<128, 2, 4, 64, 2, 0, 1>(tmA, tmB, a, n_tiles, s);
-            }
-        }
-        switch (BN) {
-            case 32: return launch_tc<32, 1, 4, 64, 2, 0, 1>(tmA, tmB, a, n_tiles, s);
-            case 64: return launch_tc<64, 1, 4, 64, 2, 0, 1>(tmA, tmB, a, n_tiles, s);
-            default: return launch_tc<128, 1, 4, 64, 2, 0, 1>(tmA, tmB, a, n_tiles, s);
-        }
-    }
-    if (ks == 3) {
-        if (by == 4) return use_cluster() ? launch_tc<64, 3, 4, 128, 4, 0, 0, 2>(tmA, tmB, a, n_tiles, s)
-                                          : launch_tc<64, 3, 4, 128, 4>(tmA, tmB, a, n_tiles, s);
-        switch (BN) {
-            case 32: return launch_tc<32, 3>(tmA, tmB, a, n_tiles, s);
-            case 64: return launch_tc<64, 3>(tmA, tmB, a, n_tiles, s);
-            default: return launch_tc<128, 3>(tmA, tmB, a, n_tiles, s);
-        }
-    }
-    if (ks == 2) {
-        switch (BN) {
-            case 32: return launch_tc<32, 2>(tmA, tmB, a, n_tiles, s);
-            case 64: return launch_tc<64, 2>(tmA, tmB, a, n_tiles, s);
-            default: return launch_tc<128, 2>(tmA, tmB, a, n_tiles, s);
-        }
-    }
-    switch (BN) {
-        case 32: return launch_tc<32, 1>(tmA, tmB, a, n_tiles, s);
-        case 64: return launch_tc<64, 1>(tmA, tmB, a, n_tiles, s);
-        default: return launch_tc<128, 1>(tmA, tmB, a, n_tiles, s);
-    }
-}
-extern "C" int sis3d_conv3d_k3_tc(const float *in, const float *w_tc, const float *bias, const float *residual, int res_ld,
-                                  int res_coff, float *out, int out_ld, int out_coff, int X, int Y, int Z, int cin, int cout,
-                                  int ks, const int32_t *tiles, int n_tiles, int act, void *stream) {
-    return conv3d_k3_tc_impl(in, w_tc, bias, residual, res_ld, res_coff, out, out_ld, out_coff, X, Y, Z, cin, cout, ks, tiles,
-                             n_tiles, act, stream, 0);
-}
-// error-compensated 3xTF32 (fp32-class accuracy on the tensor cores): w_x3 from sis3d_pack_conv_weight_tc_x3
-extern "C" int sis3d_conv3d_k3_tc_x3(const float *in, const float *w_x3, const float *bias, const float *residual, int res_ld,
-                                     int res_coff, float *out, int out_ld, int out_coff, int X, int Y, int Z, int cin, int cout,
-                                     int ks, int act, void *stream) {
-    return conv3d_k3_tc_impl(in, w_x3, bias, residual, res_ld, res_coff, out, out_ld, out_coff, X, Y, Z, cin, cout, ks, nullptr, 0,
-                             act, stream, 1);
-}
-// the same compensation with an fp16 operand split (2.5x the MMA rate): w_h3 from sis3d_pack_conv_weight_tc_h3
-extern "C" int sis3d_conv3d_k3_tc_h3(const float *in, const uint16_t *w_h3, const float *bias, const float *residual, int res_ld,
-                                     int res_coff, float *out, int out_ld, int out_coff, int X, int Y, int Z, int cin, int cout,
-                                     int ks, int act, void *stream) {
-    return conv3d_k3_tc_impl(in, (const float *)w_h3, bias, residual, res_ld, res_coff, out, out_ld, out_coff, X, Y, Z, cin, cout,
-                             ks, nullptr, 0, act, stream, 2);
-}
-// the fp16-split 1x1 conv writing split-pair activations (the A operand of sis3d_conv3d_k3_tc_fused_h3_split) instead of fp32
-extern "C" int sis3d_conv3d_k1_tc_h3_split(const float *in, const uint16_t *w_h3, const float *bias, uint16_t *out_split, int X,
-                                           int Y, int Z, int cin, int cout, int act, void *stream) {
-    if (!out_split) return SIS3D_EINVAL;
-    return conv3d_k3_tc_impl(in, (const float *)w_h3, bias, nullptr, 0, 0, nullptr, cout, 0, X, Y, Z, cin, cout, 1, nullptr, 0, act,
-                             stream, 2, (__half *)out_split);
-}
-
-// ---- bottleneck tail: 3x3x3 conv (cin -> cmid) + ReLU + 1x1 conv (cmid -> cout) + residual + act, one kernel ----------------
-extern "C" int sis3d_conv3d_k3_tc_fused_supported(int cin, int cmid, int cout) {
-    return (cin > 0 && cin % TC_KC == 0 && ((cmid == 32 && (cout == 32 || cout == 64)) || (cmid == 64 && cout == 128))) ? 1 : 0;
-}
-static int conv3d_k3_tc_fused_impl(const float *in, const float *w2_tc, const float *bias2, const float *w3_tc,
-                                   const float *bias3, const float *residual, int res_ld, int res_coff, float *out,
-                                   int out_ld, int out_coff, int X, int Y, int Z, int cin, int cmid, int cout, int act,
-                                   void *stream, int x3, bool presplit = false) {
-    if (!in || !w2_tc || !w3_tc || !out || X <= 0 || Y <= 0 || Z <= 0 || cin <= 0 || cmid <= 0 || cout <= 0) return SIS3D_EINVAL;
-    if (presplit && x3 != 2) return SIS3D_EINVAL;
-    if (!sis3d_conv3d_k3_tc_fused_supported(cin, cmid, cout)) return SIS3D_EUNSUPPORTED;
-    if (((uintptr_t)in | (uintptr_t)w2_tc | (uintptr_t)w3_tc | (uintptr_t)out) & 15) return SIS3D_EINVAL;
-    if ((out_ld | out_coff | res_ld | res_coff) & 3) return SIS3D_EINVAL;
-    EncodeTiledFn enc = get_encode();
-    if (!enc) return SIS3D_EUNSUPPORTED;
-    const int by = 2, bx = 8;
-    const int kc = x3 == 1 ? 16 : TC_KC;
-    const CUtensorMapSwizzle sw = x3 == 1 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
-    const CUtensorMapSwizzle swb = x3 == 1 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
-    const CUtensorMapSwizzle swb2 = CU_TENSOR_MAP_SWIZZLE_128B;
-    const CUtensorMapDataType dtb = x3 == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
-    const cuuint64_t wb = x3 == 2 ? 2 : 4;
-    const int halves = x3 == 1 ? 2 : 1;  // x3 = 1 weight tensors: hi rows, then lo rows
-    const int kmul = x3 == 2 ? 2 : 1;    // x3 = 2: [32 hi | 32 lo] halves per K slice in one row
-    CUtensorMap tmA, tmB, tmB2;
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    {
-        // presplit: split-pair fp16 rows, 2 cin halves per voxel (4 bytes per channel, the byte strides of fp32); a box row of
-        // 64 halves = one 32-channel slice's [hi | lo]
-        cuuint64_t dims[4] = {(cuuint64_t)cin * (presplit ? 2 : 1), (cuuint64_t)Z, (cuuint64_t)Y, (cuuint64_t)X};
-        cuuint64_t strides[3] = {(cuuint64_t)cin * 4, (cuuint64_t)Z * cin * 4, (cuuint64_t)Y * Z * cin * 4};
-        cuuint32_t box[4] = {(cuuint32_t)(presplit ? 2 * TC_KC : kc), TC_BZ, (cuuint32_t)by, (cuuint32_t)(bx + 2)};
-        if (enc(&tmA, presplit ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void *)in, dims, strides, box,
-                estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) !=
-            CUDA_SUCCESS)
-            return SIS3D_EINVAL;
-    }
-    {
-        cuuint64_t dims[2] = {(cuuint64_t)27 * cin * kmul, (cuuint64_t)cmid * halves};
-        cuuint64_t strides[1] = {dims[0] * wb};
-        cuuint32_t box[2] = {(cuuint32_t)(x3 == 2 ? 64 : kc), (cuuint32_t)cmid};
-        if (enc(&tmB, dtb, 2, (void *)w2_tc, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                swb, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-            return SIS3D_EINVAL;
-    }
-    {
-        cuuint64_t dims[2] = {(cuuint64_t)cmid * kmul, (cuuint64_t)cout * halves};
-        cuuint64_t strides[1] = {dims[0] * wb};
-        cuuint32_t box[2] = {(cuuint32_t)(TC_KC * kmul), (cuuint32_t)cout};
-        if (enc(&tmB2, dtb, 2, (void *)w3_tc, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                swb2, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-            return SIS3D_EINVAL;
-    }
-    TcArgs a;
-    a.bias = bias3; a.bias_mid = bias2; a.res = residual; a.out = out; a.tiles = nullptr; a.out16 = nullptr; a.out_split = nullptr;
-    // the main loop's weight rows (and their lo halves, x3) are indexed with the 3x3x3 conv's width, the epilogue with cout
-    a.X = X; a.Y = Y; a.Z = Z; a.cin = cin; a.cout = x3 ? cmid : cout; a.act = act;
-    a.out_ld = out_ld; a.out_coff = out_coff; a.res_ld = res_ld; a.res_coff = res_coff;
-    a.tiles_y = cdiv(Y, by); a.tiles_z = cdiv(Z, TC_BZ);
-    a.gemm_m = 0; a.gemm_chunks_per_split = 0;
-    const int n_tiles = cdiv(X, bx) * a.tiles_y * a.tiles_z;
-    cudaStream_t s = (cudaStream_t)stream;
-    if (presplit) {
-        if (cmid == 32 && cout == 32) return launch_tc<32, 3, 4, 128, 2, 32, 2, 1, true>(tmA, tmB, a, n_tiles, s, &tmB2);
-        if (cmid == 32 && cout == 64) return launch_tc<32, 3, 4, 128, 2, 64, 2, 1, true>(tmA, tmB, a, n_tiles, s, &tmB2);
-        return launch_tc<64, 3, 4, 128, 2, 128, 2, 1, true>(tmA, tmB, a, n_tiles, s, &tmB2);
-    }
-    if (x3 == 2) {
-        if (cmid == 32 && cout == 32) return launch_tc<32, 3, 4, 128, 2, 32, 2>(tmA, tmB, a, n_tiles, s, &tmB2);
-        if (cmid == 32 && cout == 64) return launch_tc<32, 3, 4, 128, 2, 64, 2>(tmA, tmB, a, n_tiles, s, &tmB2);
-        return use_cluster() ? launch_tc<64, 3, 4, 128, 2, 128, 2, 2>(tmA, tmB, a, n_tiles, s, &tmB2)
-                             : launch_tc<64, 3, 4, 128, 2, 128, 2>(tmA, tmB, a, n_tiles, s, &tmB2);
-    }
-    if (x3) {
-        if (cmid == 32 && cout == 32) return launch_tc<32, 3, 4, 64, 2, 32, 1>(tmA, tmB, a, n_tiles, s, &tmB2);
-        if (cmid == 32 && cout == 64) return launch_tc<32, 3, 4, 64, 2, 64, 1>(tmA, tmB, a, n_tiles, s, &tmB2);
-        return launch_tc<64, 3, 4, 64, 2, 128, 1>(tmA, tmB, a, n_tiles, s, &tmB2);
-    }
-    if (cmid == 32 && cout == 32) return launch_tc<32, 3, 4, 128, 2, 32>(tmA, tmB, a, n_tiles, s, &tmB2);
-    if (cmid == 32 && cout == 64) return launch_tc<32, 3, 4, 128, 2, 64>(tmA, tmB, a, n_tiles, s, &tmB2);
-    return launch_tc<64, 3, 4, 128, 2, 128>(tmA, tmB, a, n_tiles, s, &tmB2);
-}
-extern "C" int sis3d_conv3d_k3_tc_fused(const float *in, const float *w2_tc, const float *bias2, const float *w3_tc,
-                                        const float *bias3, const float *residual, int res_ld, int res_coff, float *out,
-                                        int out_ld, int out_coff, int X, int Y, int Z, int cin, int cmid, int cout, int act,
-                                        void *stream) {
-    return conv3d_k3_tc_fused_impl(in, w2_tc, bias2, w3_tc, bias3, residual, res_ld, res_coff, out, out_ld, out_coff, X, Y, Z, cin,
-                                   cmid, cout, act, stream, 0);
-}
-extern "C" int sis3d_conv3d_k3_tc_fused_x3(const float *in, const float *w2_x3, const float *bias2, const float *w3_x3,
-                                           const float *bias3, const float *residual, int res_ld, int res_coff, float *out,
-                                           int out_ld, int out_coff, int X, int Y, int Z, int cin, int cmid, int cout, int act,
-                                           void *stream) {
-    return conv3d_k3_tc_fused_impl(in, w2_x3, bias2, w3_x3, bias3, residual, res_ld, res_coff, out, out_ld, out_coff, X, Y, Z, cin,
-                                   cmid, cout, act, stream, 1);
-}
-extern "C" int sis3d_conv3d_k3_tc_fused_h3(const float *in, const uint16_t *w2_h3, const float *bias2, const uint16_t *w3_h3,
-                                           const float *bias3, const float *residual, int res_ld, int res_coff, float *out,
-                                           int out_ld, int out_coff, int X, int Y, int Z, int cin, int cmid, int cout, int act,
-                                           void *stream) {
-    return conv3d_k3_tc_fused_impl(in, (const float *)w2_h3, bias2, (const float *)w3_h3, bias3, residual, res_ld, res_coff, out,
-                                   out_ld, out_coff, X, Y, Z, cin, cmid, cout, act, stream, 2);
-}
-// the same tail fed split-pair activations (from sis3d_conv3d_k1_tc_h3_split): no operand split on the SM, same result bits
-extern "C" int sis3d_conv3d_k3_tc_fused_h3_split(const uint16_t *in_split, const uint16_t *w2_h3, const float *bias2,
-                                                 const uint16_t *w3_h3, const float *bias3, const float *residual, int res_ld,
-                                                 int res_coff, float *out, int out_ld, int out_coff, int X, int Y, int Z, int cin,
-                                                 int cmid, int cout, int act, void *stream) {
-    return conv3d_k3_tc_fused_impl((const float *)in_split, (const float *)w2_h3, bias2, (const float *)w3_h3, bias3, residual,
-                                   res_ld, res_coff, out, out_ld, out_coff, X, Y, Z, cin, cmid, cout, act, stream, 2, true);
-}
-
-// ---- y[M][N] = act(x[M][K] . w[N][K]^T + b): fully connected layer on the tensor cores (TF32), split-K ------------
-static int gemm_tc_splits(int M, int N, int K, int kc) {
-    const int tiles = cdiv(M, TC_BM) * (N / (N >= 128 ? 128 : N));
-    const int chunks = K / kc;
-    int splits = max(1, min(chunks / (128 / kc), (kNumSMs + tiles - 1) / tiles));
-    return splits;
-}
-extern "C" int sis3d_linear_tc_supported(int K, int N) {
-    return (K > 0 && N > 0 && K % TC_KC == 0 && (N == 32 || N == 64 || N % 128 == 0)) ? 1 : 0;
-}
-extern "C" size_t sis3d_linear_tc_workspace_bytes(int M, int N, int K) {
-    if (M <= 0 || !sis3d_linear_tc_supported(K, N)) return 0;  // gemm_tc_splits divides by the tile and chunk counts
-    return sizeof(float) * (size_t)gemm_tc_splits(M, N, K, 16) * M * N + 16;  // the x3 variant splits K finer: covers both
-}
-static int linear_tc_impl(const float *x, const float *w_nk, const float *bias, float *y, int M, int K, int N, int act,
-                          void *workspace, size_t workspace_bytes, void *stream, int x3) {
-    if (!x || !w_nk || !y || !workspace || M <= 0 || K <= 0 || N <= 0) return SIS3D_EINVAL;
-    if (!sis3d_linear_tc_supported(K, N)) return SIS3D_EUNSUPPORTED;
-    if (((uintptr_t)x | (uintptr_t)w_nk | (uintptr_t)workspace) & 15) return SIS3D_EINVAL;
-    EncodeTiledFn enc = get_encode();
-    if (!enc) return SIS3D_EUNSUPPORTED;
-    const int BN = N >= 128 ? 128 : N;
-    const int kc = x3 == 1 ? 16 : TC_KC;
-    const CUtensorMapSwizzle sw = x3 == 1 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
-    const CUtensorMapSwizzle swb = x3 == 1 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
-    const CUtensorMapDataType dtb = x3 == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
-    int splits = gemm_tc_splits(M, N, K, kc);
-    const int chunks = K / kc;
-    const int per = cdiv(chunks, splits);
-    splits = cdiv(chunks, per);
-    // the documented size, not this mode's need: a buffer that is too small for the finest split is rejected in every mode
-    if (workspace_bytes < sis3d_linear_tc_workspace_bytes(M, N, K)) return SIS3D_EWORKSPACE;
-    CUtensorMap tmA, tmB;
-    {
-        cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)M};
-        cuuint64_t strides[1] = {(cuuint64_t)K * 4};
-        cuuint32_t box[2] = {(cuuint32_t)kc, TC_BM};
-        cuuint32_t estr[2] = {1, 1};
-        if (enc(&tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void *)x, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-            return SIS3D_EINVAL;
-        cuuint64_t dimsb[2] = {(cuuint64_t)K * (x3 == 2 ? 2 : 1), (cuuint64_t)N * (x3 == 1 ? 2 : 1)};
-        cuuint64_t stridesb[1] = {dimsb[0] * (x3 == 2 ? 2 : 4)};
-        cuuint32_t boxb[2] = {(cuuint32_t)(x3 == 2 ? 64 : kc), (cuuint32_t)BN};
-        if (enc(&tmB, dtb, 2, (void *)w_nk, dimsb, stridesb, boxb, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                swb, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-            return SIS3D_EINVAL;
-    }
-    TcArgs a = {};
-    a.out = (float *)workspace; a.out_ld = N; a.cin = K; a.cout = N; a.gemm_m = M; a.gemm_chunks_per_split = per;
-    cudaStream_t s = (cudaStream_t)stream;
-    const int mt = cdiv(M, TC_BM);
-    int rc;
-    if (x3 == 2) {
-        rc = BN == 32 ? launch_tc<32, 0, 4, 128, 2, 0, 2>(tmA, tmB, a, mt, s, nullptr, splits)
-           : BN == 64 ? launch_tc<64, 0, 4, 128, 2, 0, 2>(tmA, tmB, a, mt, s, nullptr, splits)
-                      : launch_tc<128, 0, 4, 128, 2, 0, 2>(tmA, tmB, a, mt, s, nullptr, splits);
-    } else if (x3) {
-        rc = BN == 32 ? launch_tc<32, 0, 4, 64, 2, 0, 1>(tmA, tmB, a, mt, s, nullptr, splits)
-           : BN == 64 ? launch_tc<64, 0, 4, 64, 2, 0, 1>(tmA, tmB, a, mt, s, nullptr, splits)
-                      : launch_tc<128, 0, 4, 64, 2, 0, 1>(tmA, tmB, a, mt, s, nullptr, splits);
-    } else {
-        rc = BN == 32 ? launch_tc<32, 0>(tmA, tmB, a, mt, s, nullptr, splits)
-           : BN == 64 ? launch_tc<64, 0>(tmA, tmB, a, mt, s, nullptr, splits)
-                      : launch_tc<128, 0>(tmA, tmB, a, mt, s, nullptr, splits);
-    }
-    if (rc) return rc;
-    gemm_splitk_reduce_kernel<<<cdiv(M * N, 256), 256, 0, s>>>((const float *)workspace, splits, (int64_t)M * N, bias, y, M, N, act);
-    return finish_launch();
-}
-extern "C" int sis3d_linear_tc(const float *x, const float *w_nk, const float *bias, float *y, int M, int K, int N, int act,
-                               void *workspace, size_t workspace_bytes, void *stream) {
-    return linear_tc_impl(x, w_nk, bias, y, M, K, N, act, workspace, workspace_bytes, stream, 0);
-}
-// w_x3 = sis3d_pack_conv_weight_tc_x3(w[N][K] viewed as a 1x1 conv): [2][N][K]
-extern "C" int sis3d_linear_tc_x3(const float *x, const float *w_x3, const float *bias, float *y, int M, int K, int N, int act,
-                                  void *workspace, size_t workspace_bytes, void *stream) {
-    return linear_tc_impl(x, w_x3, bias, y, M, K, N, act, workspace, workspace_bytes, stream, 1);
-}
-extern "C" int sis3d_linear_tc_h3(const float *x, const uint16_t *w_h3, const float *bias, float *y, int M, int K, int N, int act,
-                                  void *workspace, size_t workspace_bytes, void *stream) {
-    return linear_tc_impl(x, (const float *)w_h3, bias, y, M, K, N, act, workspace, workspace_bytes, stream, 2);
-}
-
 // ---- fp16-operand variant (f16 wgmma): activations and weights stored as fp16, fp32 accumulation in registers ------
 extern "C" int sis3d_pack_conv_weight_tc_f16(const float *w, int cout, int cin, int ks, uint16_t *w16, void *stream) {
     if (!w || !w16 || cout <= 0 || cin <= 0 || (ks != 1 && ks != 3)) return SIS3D_EINVAL;
@@ -1193,73 +848,341 @@ extern "C" int sis3d_cast_f16(const float *in, int in_ld, int in_coff, int64_t r
     cast_f16_kernel<<<(int)imin64(cdiv64(rows * (C / 4), 256), kNumSMs * 8), 256, 0, (cudaStream_t)stream>>>(in, in_ld, in_coff, rows, C / 4, (__half *)out);
     return finish_launch();
 }
+
+// ---- launching the tensor-core kernel -------------------------------------------------------------------------------
+// Operand form of the math modes: one TF32 product, the TF32 split (x3), the fp16 split (h3) with fp32 or pre-split input,
+// and fp16 operands (f16).
+enum TcForm { TC_TF32, TC_TF32_SPLIT, TC_F16_SPLIT, TC_F16_PRESPLIT, TC_F16 };
+
+// A (activations, GEMM rows) and B (weights) of every form carry eb bytes per K index (channel x tap), so one K slice of
+// kc channels is one kc * eb-byte shared-memory row of either operand (ROWB), and every TMA box row is one swizzle span.
+struct TcOperands {
+    int kc, eb, x3;                // K slice width; EB; X3 (0: one product, 1: TF32 split, 2: fp16 split)
+    bool ps;                       // PS: A holds split pairs, 32 hi then 32 lo halves per 32-channel slice
+    CUtensorMapDataType adt, wdt;  // element types of A and of the packed weights in global memory
+    int wrows;                     // weight rows per output channel (TF32 split: hi rows, then lo rows)
+    int bn_max;                    // widest N tile
+};
+static TcOperands tc_operands(TcForm form, int cin) {
+    const CUtensorMapDataType F32 = CU_TENSOR_MAP_DATA_TYPE_FLOAT32, F16 = CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+    switch (form) {
+        case TC_TF32: return {TC_KC, 4, 0, false, F32, F32, 1, 128};
+        case TC_TF32_SPLIT: return {16, 4, 1, false, F32, F32, 2, 128};  // 64-byte K rows, so hi + lo tiles fit the same smem
+        case TC_F16_SPLIT: return {TC_KC, 4, 2, false, F32, F16, 1, 128};  // weight rows: [32 hi | 32 lo] halves per K slice
+        case TC_F16_PRESPLIT: return {TC_KC, 4, 2, true, F16, F16, 1, 128};
+        default:  // fp16 operands: cin % 64 == 0 in 128-byte rows; cin == 32 in 64-byte rows, with N tiles of at most 64
+            if (cin % 64 == 0) return {64, 2, 0, false, F16, F16, 1, 128};
+            return {32, 2, 0, false, F16, F16, 1, 64};
+    }
+}
+static int tc_block_n(const TcOperands &op, int cout) { return cout < op.bn_max ? cout : op.bn_max; }
+// explicit tile lists (ragged RoI crops) of 64 -> 64 3x3x3 layers use 4x4x8 bricks, everything else 8x2x8 (x, y, z)
+static int tc_brick_y(bool tiles, int ks, int cin, int cout) { return tiles && ks == 3 && cout == 64 && cin % 64 == 0 ? 4 : 2; }
+
+static CUtensorMapSwizzle tc_swizzle(uint32_t row_bytes) {
+    return row_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
+}
+static uint32_t tc_elem_bytes(CUtensorMapDataType dt) { return dt == CU_TENSOR_MAP_DATA_TYPE_FLOAT16 ? 2 : 4; }
+// dense channels-last activation [X][Y][Z][vb bytes]; a box is row_bytes of channels by bz x by x bx voxels, taking every
+// sd-th voxel (sd = 2: the 2x2x2 stride-2 conv)
+static bool tmap_act(EncodeTiledFn enc, CUtensorMap *m, CUtensorMapDataType dt, const void *p, int X, int Y, int Z, uint64_t vb,
+                     uint32_t row_bytes, uint32_t bz, uint32_t by, uint32_t bx, uint32_t sd) {
+    const uint32_t e = tc_elem_bytes(dt);
+    cuuint64_t dims[4] = {vb / e, (cuuint64_t)Z, (cuuint64_t)Y, (cuuint64_t)X};
+    cuuint64_t strides[3] = {vb, (cuuint64_t)Z * vb, (cuuint64_t)Y * Z * vb};
+    // with element strides the box is given in traversed elements: N loaded voxels = boxDim / stride
+    cuuint32_t box[4] = {row_bytes / e, bz * sd, by * sd, bx * sd};
+    cuuint32_t estr[4] = {1, sd, sd, sd};
+    return enc(m, dt, 4, (void *)p, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, tc_swizzle(row_bytes),
+               CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+// row-major matrix [rows][rb bytes] (weights, W3, GEMM A); a box is row_bytes by box_rows rows
+static bool tmap_matrix(EncodeTiledFn enc, CUtensorMap *m, CUtensorMapDataType dt, const void *p, uint64_t rb, uint64_t rows,
+                        uint32_t row_bytes, uint32_t box_rows, CUtensorMapL2promotion l2) {
+    const uint32_t e = tc_elem_bytes(dt);
+    cuuint64_t dims[2] = {rb / e, rows}, strides[1] = {rb};
+    cuuint32_t box[2] = {row_bytes / e, box_rows}, estr[2] = {1, 1};
+    return enc(m, dt, 2, (void *)p, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, tc_swizzle(row_bytes), l2,
+               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+// SIS3D_CLUSTER=1 turns the 2-CTA weight-tile multicast ON (off by default: multicast halves the weight bytes each SM
+// fetches, but not the rate at which an SM receives TMA rows; kept as an A/B switch)
+static bool use_cluster() {
+    static const bool on = getenv("SIS3D_CLUSTER") != nullptr && getenv("SIS3D_CLUSTER")[0] == '1';
+    return on;
+}
+
+// Every instance of the kernel, each listed once (tests/test_tc_instance_coverage.py reads this list): runs instance t
+static int tc_launch(TcInst t, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmB2, const TcArgs &a,
+                     cudaStream_t s, int grid_z) {
+    int rc = SIS3D_EUNSUPPORTED;
+    if (use_cluster()) {  // the layers with a 2-CTA twin run it
+        t.cl = 2;
+        if (launch_tc<128, 3, 4, 128, 2, 0, 2, 2, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+        if (launch_tc<64, 3, 4, 128, 4, 0, 0, 2, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+        if (launch_tc<64, 3, 2, 128, 4, 0, 0, 2, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+        if (launch_tc<64, 3, 4, 128, 2, 128, 2, 2, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+        t.cl = 1;
+    }
+    // convs (BN, KS): TF32, TF32 split, fp16 split; the TF32 4x4x8-brick tile-list layer
+    if (launch_tc<32, 3, 4, 128, 2, 0, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<64, 3, 4, 128, 2, 0, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<128, 3, 4, 128, 2, 0, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<32, 2, 4, 128, 2, 0, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<64, 2, 4, 128, 2, 0, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<128, 2, 4, 128, 2, 0, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<32, 1, 4, 128, 2, 0, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<64, 1, 4, 128, 2, 0, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<128, 1, 4, 128, 2, 0, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<32, 3, 4, 64, 2, 0, 1, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<64, 3, 4, 64, 2, 0, 1, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<128, 3, 4, 64, 2, 0, 1, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<32, 2, 4, 64, 2, 0, 1, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<64, 2, 4, 64, 2, 0, 1, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<128, 2, 4, 64, 2, 0, 1, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<32, 1, 4, 64, 2, 0, 1, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<64, 1, 4, 64, 2, 0, 1, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<128, 1, 4, 64, 2, 0, 1, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<32, 3, 4, 128, 2, 0, 2, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<64, 3, 4, 128, 2, 0, 2, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<128, 3, 4, 128, 2, 0, 2, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<32, 2, 4, 128, 2, 0, 2, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<64, 2, 4, 128, 2, 0, 2, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<128, 2, 4, 128, 2, 0, 2, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<32, 1, 4, 128, 2, 0, 2, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<64, 1, 4, 128, 2, 0, 2, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<128, 1, 4, 128, 2, 0, 2, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<64, 3, 4, 128, 4, 0, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    // fused tails (cmid, cout): TF32, TF32 split, fp16 split, fp16 split on split-pair input
+    if (launch_tc<32, 3, 4, 128, 2, 32, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<32, 3, 4, 128, 2, 64, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<64, 3, 4, 128, 2, 128, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<32, 3, 4, 64, 2, 32, 1, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<32, 3, 4, 64, 2, 64, 1, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<64, 3, 4, 64, 2, 128, 1, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<32, 3, 4, 128, 2, 32, 2, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<32, 3, 4, 128, 2, 64, 2, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<64, 3, 4, 128, 2, 128, 2, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<32, 3, 4, 128, 2, 32, 2, 1, true>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<32, 3, 4, 128, 2, 64, 2, 1, true>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<64, 3, 4, 128, 2, 128, 2, 1, true>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    // GEMMs (BN): TF32, TF32 split, fp16 split
+    if (launch_tc<32, 0, 4, 128, 2, 0, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<64, 0, 4, 128, 2, 0, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<128, 0, 4, 128, 2, 0, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<32, 0, 4, 64, 2, 0, 1, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<64, 0, 4, 64, 2, 0, 1, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<128, 0, 4, 64, 2, 0, 1, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<32, 0, 4, 128, 2, 0, 2, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<64, 0, 4, 128, 2, 0, 2, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<128, 0, 4, 128, 2, 0, 2, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    // fp16-operand convs (BN, KS): 128-byte rows, the 4x4x8-brick tile-list layer, 64-byte rows
+    if (launch_tc<32, 3, 2, 128, 2, 0, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<64, 3, 2, 128, 2, 0, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<128, 3, 2, 128, 2, 0, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<32, 1, 2, 128, 2, 0, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<64, 1, 2, 128, 2, 0, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<128, 1, 2, 128, 2, 0, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<64, 3, 2, 128, 4, 0, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<32, 3, 2, 64, 2, 0, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<64, 3, 2, 64, 2, 0, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<32, 1, 2, 64, 2, 0, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    if (launch_tc<64, 1, 2, 64, 2, 0, 0, 1, false>(t, tmA, tmB, tmB2, a, s, grid_z, rc)) return rc;
+    return rc;
+}
+
+extern "C" int sis3d_conv3d_k3_tc_fused_supported(int cin, int cmid, int cout) {
+    return (cin > 0 && cin % TC_KC == 0 && ((cmid == 32 && (cout == 32 || cout == 64)) || (cmid == 64 && cout == 128))) ? 1 : 0;
+}
+extern "C" int sis3d_linear_tc_supported(int K, int N) { return sis3d_conv3d_k3_tc_supported(K, N); }
+static int gemm_tc_splits(int M, int N, int K, const TcOperands &op) {
+    const int tiles = cdiv(M, TC_BM) * (N / tc_block_n(op, N));
+    const int chunks = K / op.kc;
+    return max(1, min(chunks / (128 / op.kc), (kNumSMs + tiles - 1) / tiles));
+}
+extern "C" size_t sis3d_linear_tc_workspace_bytes(int M, int N, int K) {
+    if (M <= 0 || !sis3d_linear_tc_supported(K, N)) return 0;  // gemm_tc_splits divides by the tile and chunk counts
+    // the TF32 split's 16-channel K slices split K finest: covers every mode
+    return sizeof(float) * (size_t)gemm_tc_splits(M, N, K, tc_operands(TC_TF32_SPLIT, K)) * M * N + 16;
+}
+
+// One launch as an entry point describes it.  The fields up to `stream` follow sis3d_conv3d_k3_tc's arguments.
+enum TcOp { TC_CONV, TC_FUSED, TC_GEMM };
+struct TcLaunch {
+    TcOp op;
+    TcForm form;
+    const void *in, *w;
+    const float *bias, *res;
+    int res_ld, res_coff;
+    float *out;                                    // GEMM: y
+    int out_ld, out_coff, X, Y, Z, cin, cout, ks;  // GEMM: X = M, Y = Z = 1, cin = K, cout = N, ks = 1
+    const int32_t *tiles;
+    int n_tiles, act;
+    void *stream;
+    void *workspace;          // GEMM: split-K partial sums, reduced into y
+    size_t workspace_bytes;
+    const void *w3;           // fused tail: the 1x1 conv's weights, its input width and the 3x3x3 conv's bias
+    int cmid;
+    const float *bias_mid;
+    __half *out16, *out_split;
+};
+
+static int tc_run(const TcLaunch &L) {
+    const bool fused = L.op == TC_FUSED, gemm = L.op == TC_GEMM;
+    // argument checks, in the order that decides which code a call with several faults gets
+    if (!L.in || !L.w || !(L.out || L.out16 || L.out_split) || (fused && !L.w3) || (gemm && !L.workspace) || L.X <= 0 ||
+        L.Y <= 0 || L.Z <= 0 || L.cin <= 0 || L.cout <= 0 || (fused && L.cmid <= 0) ||
+        !(L.ks == 1 || L.ks == 3 || (L.ks == 2 && L.form != TC_F16)))
+        return SIS3D_EINVAL;
+    if (L.out_split && (L.cout % TC_KC || ((uintptr_t)L.out_split & 15))) return SIS3D_EINVAL;
+    if (L.ks == 2 && (L.tiles || L.X < 2 || L.Y < 2 || L.Z < 2)) return SIS3D_EINVAL;
+    if (!(fused ? sis3d_conv3d_k3_tc_fused_supported(L.cin, L.cmid, L.cout) : sis3d_conv3d_k3_tc_supported(L.cin, L.cout)))
+        return SIS3D_EUNSUPPORTED;
+    // TMA reads and the kernel's vector stores need 16-byte alignment; the GEMM's y is written by the scalar reduce
+    if (((uintptr_t)L.in | (uintptr_t)L.w | (uintptr_t)L.w3 | (uintptr_t)(gemm ? L.workspace : L.out) | (uintptr_t)L.out16) & 15)
+        return SIS3D_EINVAL;
+    if ((L.out_ld | L.out_coff | L.res_ld | L.res_coff) & 3) return SIS3D_EINVAL;
+    const TcOperands op = tc_operands(L.form, L.cin);
+    if (L.form == TC_F16 && op.kc == 32 && L.cin != 32) return SIS3D_EUNSUPPORTED;  // fp16 rows: 32 or a multiple of 64 channels
+    EncodeTiledFn enc = get_encode();
+    if (!enc) return SIS3D_EUNSUPPORTED;
+
+    const int rowb = op.kc * op.eb, taps = L.ks * L.ks * L.ks;
+    const int by = tc_brick_y(L.tiles, L.ks, L.cin, L.cout), bx = 16 / by;
+    const int width = fused ? L.cmid : L.cout;  // the weight rows of the main loop (the fused tail's 3x3x3 conv)
+    const int BN = tc_block_n(op, width);
+    int splits = 1, per = 0;
+    if (gemm) {
+        splits = gemm_tc_splits(L.X, L.cout, L.cin, op);
+        const int chunks = L.cin / op.kc;
+        per = cdiv(chunks, splits);
+        splits = cdiv(chunks, per);
+        // the documented size, not this mode's need: a buffer that is too small for the finest split is rejected in every mode
+        if (L.workspace_bytes < sis3d_linear_tc_workspace_bytes(L.X, L.cout, L.cin)) return SIS3D_EWORKSPACE;
+    }
+    const int sd = L.ks == 2 ? 2 : 1;                       // ks == 2 is the stride-2, pad-0 conv: X, Y, Z are the INPUT extents
+    const int Xo = L.X / sd, Yo = L.Y / sd, Zo = L.Z / sd;  // output extents (floor, as nn.Conv3d)
+    const uint64_t kb = (uint64_t)L.cin * op.eb;            // bytes of A per voxel (GEMM row), of B per tap and output channel
+    const CUtensorMapL2promotion l2w = CU_TENSOR_MAP_L2_PROMOTION_L2_256B;
+    CUtensorMap tmA, tmB, tmB2;
+    if (!(gemm ? tmap_matrix(enc, &tmA, op.adt, L.in, kb, L.X, rowb, TC_BM, CU_TENSOR_MAP_L2_PROMOTION_L2_128B)
+               : tmap_act(enc, &tmA, op.adt, L.in, L.X, L.Y, L.Z, kb, rowb, TC_BZ, by, L.ks == 3 ? bx + 2 : bx, sd)) ||
+        !tmap_matrix(enc, &tmB, op.wdt, L.w, taps * kb, (uint64_t)width * op.wrows, rowb, BN, l2w) ||
+        (fused && !tmap_matrix(enc, &tmB2, op.wdt, L.w3, (uint64_t)L.cmid * op.eb, (uint64_t)L.cout * op.wrows, TC_KC * op.eb,
+                               L.cout, l2w)))
+        return SIS3D_EINVAL;
+
+    TcArgs a = {};
+    a.n_tiles = L.n_tiles;
+    if (gemm) {
+        a.out = (float *)L.workspace; a.out_ld = L.cout; a.cin = L.cin; a.cout = L.cout;
+        a.gemm_m = L.X; a.gemm_chunks_per_split = per; a.n_tiles = cdiv(L.X, TC_BM);
+    } else {
+        a.bias = L.bias; a.bias_mid = L.bias_mid; a.res = L.res; a.out = L.out; a.out16 = L.out16; a.out_split = L.out_split;
+        a.tiles = L.tiles;
+        // the fused tail's compensated main loop indexes weight rows (and their lo halves) with cmid, the epilogue with cout
+        a.X = Xo; a.Y = Yo; a.Z = Zo; a.cin = L.cin; a.cout = fused && op.x3 ? L.cmid : L.cout; a.act = L.act;
+        a.out_ld = L.out_ld; a.out_coff = L.out_coff; a.res_ld = L.res_ld; a.res_coff = L.res_coff;
+        a.tiles_y = cdiv(Yo, by); a.tiles_z = cdiv(Zo, TC_BZ);
+        if (!L.tiles) a.n_tiles = cdiv(Xo, bx) * a.tiles_y * a.tiles_z;
+    }
+    if (a.n_tiles <= 0) return SIS3D_OK;
+    cudaStream_t s = (cudaStream_t)L.stream;
+    const TcInst t = {BN, gemm ? 0 : L.ks, op.eb, rowb, by, fused ? L.cout : 0, op.x3, 1, op.ps};
+    const int rc = tc_launch(t, tmA, tmB, fused ? tmB2 : tmB, a, s, splits);
+    if (rc || !gemm) return rc;
+    gemm_splitk_reduce_kernel<<<cdiv(L.X * L.cout, 256), 256, 0, s>>>((const float *)L.workspace, splits, (int64_t)L.X * L.cout,
+                                                                       L.bias, L.out, L.X, L.cout, L.act);
+    return finish_launch();
+}
+
+extern "C" int sis3d_conv3d_k3_tc(const float *in, const float *w_tc, const float *bias, const float *residual, int res_ld,
+                                  int res_coff, float *out, int out_ld, int out_coff, int X, int Y, int Z, int cin, int cout,
+                                  int ks, const int32_t *tiles, int n_tiles, int act, void *stream) {
+    return tc_run({TC_CONV, TC_TF32, in, w_tc, bias, residual, res_ld, res_coff, out, out_ld, out_coff, X, Y, Z, cin, cout, ks,
+                   tiles, n_tiles, act, stream});
+}
+// error-compensated 3xTF32 (fp32-class accuracy on the tensor cores): w_x3 from sis3d_pack_conv_weight_tc_x3
+extern "C" int sis3d_conv3d_k3_tc_x3(const float *in, const float *w_x3, const float *bias, const float *residual, int res_ld,
+                                     int res_coff, float *out, int out_ld, int out_coff, int X, int Y, int Z, int cin, int cout,
+                                     int ks, int act, void *stream) {
+    return tc_run({TC_CONV, TC_TF32_SPLIT, in, w_x3, bias, residual, res_ld, res_coff, out, out_ld, out_coff, X, Y, Z, cin, cout,
+                   ks, nullptr, 0, act, stream});
+}
+// the same compensation with an fp16 operand split (2.5x the MMA rate): w_h3 from sis3d_pack_conv_weight_tc_h3
+extern "C" int sis3d_conv3d_k3_tc_h3(const float *in, const uint16_t *w_h3, const float *bias, const float *residual, int res_ld,
+                                     int res_coff, float *out, int out_ld, int out_coff, int X, int Y, int Z, int cin, int cout,
+                                     int ks, int act, void *stream) {
+    return tc_run({TC_CONV, TC_F16_SPLIT, in, w_h3, bias, residual, res_ld, res_coff, out, out_ld, out_coff, X, Y, Z, cin, cout,
+                   ks, nullptr, 0, act, stream});
+}
+// the fp16-split 1x1 conv writing split-pair activations (the A operand of sis3d_conv3d_k3_tc_fused_h3_split) instead of fp32
+extern "C" int sis3d_conv3d_k1_tc_h3_split(const float *in, const uint16_t *w_h3, const float *bias, uint16_t *out_split, int X,
+                                           int Y, int Z, int cin, int cout, int act, void *stream) {
+    return tc_run({TC_CONV, TC_F16_SPLIT, in, w_h3, bias, nullptr, 0, 0, nullptr, cout, 0, X, Y, Z, cin, cout, 1, nullptr, 0, act,
+                   stream, nullptr, 0, nullptr, 0, nullptr, nullptr, (__half *)out_split});
+}
+
+// ---- bottleneck tail: 3x3x3 conv (cin -> cmid) + ReLU + 1x1 conv (cmid -> cout) + residual + act, one kernel ----------------
+extern "C" int sis3d_conv3d_k3_tc_fused(const float *in, const float *w2_tc, const float *bias2, const float *w3_tc,
+                                        const float *bias3, const float *residual, int res_ld, int res_coff, float *out,
+                                        int out_ld, int out_coff, int X, int Y, int Z, int cin, int cmid, int cout, int act,
+                                        void *stream) {
+    return tc_run({TC_FUSED, TC_TF32, in, w2_tc, bias3, residual, res_ld, res_coff, out, out_ld, out_coff, X, Y, Z, cin, cout, 3,
+                   nullptr, 0, act, stream, nullptr, 0, w3_tc, cmid, bias2});
+}
+extern "C" int sis3d_conv3d_k3_tc_fused_x3(const float *in, const float *w2_x3, const float *bias2, const float *w3_x3,
+                                           const float *bias3, const float *residual, int res_ld, int res_coff, float *out,
+                                           int out_ld, int out_coff, int X, int Y, int Z, int cin, int cmid, int cout, int act,
+                                           void *stream) {
+    return tc_run({TC_FUSED, TC_TF32_SPLIT, in, w2_x3, bias3, residual, res_ld, res_coff, out, out_ld, out_coff, X, Y, Z, cin,
+                   cout, 3, nullptr, 0, act, stream, nullptr, 0, w3_x3, cmid, bias2});
+}
+extern "C" int sis3d_conv3d_k3_tc_fused_h3(const float *in, const uint16_t *w2_h3, const float *bias2, const uint16_t *w3_h3,
+                                           const float *bias3, const float *residual, int res_ld, int res_coff, float *out,
+                                           int out_ld, int out_coff, int X, int Y, int Z, int cin, int cmid, int cout, int act,
+                                           void *stream) {
+    return tc_run({TC_FUSED, TC_F16_SPLIT, in, w2_h3, bias3, residual, res_ld, res_coff, out, out_ld, out_coff, X, Y, Z, cin,
+                   cout, 3, nullptr, 0, act, stream, nullptr, 0, w3_h3, cmid, bias2});
+}
+// the same tail fed split-pair activations (from sis3d_conv3d_k1_tc_h3_split): no operand split on the SM, same result bits
+extern "C" int sis3d_conv3d_k3_tc_fused_h3_split(const uint16_t *in_split, const uint16_t *w2_h3, const float *bias2,
+                                                 const uint16_t *w3_h3, const float *bias3, const float *residual, int res_ld,
+                                                 int res_coff, float *out, int out_ld, int out_coff, int X, int Y, int Z, int cin,
+                                                 int cmid, int cout, int act, void *stream) {
+    return tc_run({TC_FUSED, TC_F16_PRESPLIT, in_split, w2_h3, bias3, residual, res_ld, res_coff, out, out_ld, out_coff, X, Y, Z,
+                   cin, cout, 3, nullptr, 0, act, stream, nullptr, 0, w3_h3, cmid, bias2});
+}
+
+// ---- y[M][N] = act(x[M][K] . w[N][K]^T + b): fully connected layer on the tensor cores, split-K ------------
+extern "C" int sis3d_linear_tc(const float *x, const float *w_nk, const float *bias, float *y, int M, int K, int N, int act,
+                               void *workspace, size_t workspace_bytes, void *stream) {
+    return tc_run({TC_GEMM, TC_TF32, x, w_nk, bias, nullptr, 0, 0, y, 0, 0, M, 1, 1, K, N, 1, nullptr, 0, act, stream,
+                   workspace, workspace_bytes});
+}
+// w_x3 = sis3d_pack_conv_weight_tc_x3(w[N][K] viewed as a 1x1 conv): [2][N][K]
+extern "C" int sis3d_linear_tc_x3(const float *x, const float *w_x3, const float *bias, float *y, int M, int K, int N, int act,
+                                  void *workspace, size_t workspace_bytes, void *stream) {
+    return tc_run({TC_GEMM, TC_TF32_SPLIT, x, w_x3, bias, nullptr, 0, 0, y, 0, 0, M, 1, 1, K, N, 1, nullptr, 0, act, stream,
+                   workspace, workspace_bytes});
+}
+extern "C" int sis3d_linear_tc_h3(const float *x, const uint16_t *w_h3, const float *bias, float *y, int M, int K, int N, int act,
+                                  void *workspace, size_t workspace_bytes, void *stream) {
+    return tc_run({TC_GEMM, TC_F16_SPLIT, x, w_h3, bias, nullptr, 0, 0, y, 0, 0, M, 1, 1, K, N, 1, nullptr, 0, act, stream,
+                   workspace, workspace_bytes});
+}
+
 extern "C" int sis3d_conv3d_tc_f16(const uint16_t *in16, const uint16_t *w16, const float *bias, const float *residual,
                                    int res_ld, int res_coff, float *out32, uint16_t *out16, int out_ld, int out_coff, int X, int Y,
                                    int Z, int cin, int cout, int ks, const int32_t *tiles, int n_tiles, int act, void *stream) {
-    if (!in16 || !w16 || (!out32 && !out16) || X <= 0 || Y <= 0 || Z <= 0 || cin <= 0 || cout <= 0 || (ks != 1 && ks != 3))
-        return SIS3D_EINVAL;
-    const int taps = ks * ks * ks;
-    if (!sis3d_conv3d_k3_tc_supported(cin, cout)) return SIS3D_EUNSUPPORTED;
-    if (((uintptr_t)in16 | (uintptr_t)w16 | (uintptr_t)out32 | (uintptr_t)out16) & 15) return SIS3D_EINVAL;
-    if ((out_ld | out_coff | res_ld | res_coff) & 3) return SIS3D_EINVAL;
-    EncodeTiledFn enc = get_encode();
-    if (!enc) return SIS3D_EUNSUPPORTED;
-    const bool wide = cin % 64 == 0;       // 64 channels = 128 B rows; C_in = 32 -> 64 B rows (SWIZZLE_64B)
-    const int BN = wide ? (cout >= 128 ? 128 : cout) : (cout >= 64 ? 64 : cout);  // 64-B rows: N tiles of at most 64
-    const int kc = wide ? 64 : 32;
-    if (!wide && cin != 32) return SIS3D_EUNSUPPORTED;
-    const int by = (tiles && ks == 3 && cout == 64 && wide) ? 4 : 2, bx = 16 / by;
-    const CUtensorMapSwizzle sw = wide ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-    CUtensorMap tmA, tmB;
-    {
-        cuuint64_t dims[4] = {(cuuint64_t)cin, (cuuint64_t)Z, (cuuint64_t)Y, (cuuint64_t)X};
-        cuuint64_t strides[3] = {(cuuint64_t)cin * 2, (cuuint64_t)Z * cin * 2, (cuuint64_t)Y * Z * cin * 2};
-        cuuint32_t box[4] = {(cuuint32_t)kc, TC_BZ, (cuuint32_t)by, (cuuint32_t)(ks == 3 ? bx + 2 : bx)};
-        cuuint32_t estr[4] = {1, 1, 1, 1};
-        if (enc(&tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, (void *)in16, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
-                CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-            return SIS3D_EINVAL;
-    }
-    {
-        cuuint64_t dims[2] = {(cuuint64_t)taps * cin, (cuuint64_t)cout};
-        cuuint64_t strides[1] = {(cuuint64_t)taps * cin * 2};
-        cuuint32_t box[2] = {(cuuint32_t)kc, (cuuint32_t)BN};
-        cuuint32_t estr[2] = {1, 1};
-        if (enc(&tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void *)w16, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
-                CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-            return SIS3D_EINVAL;
-    }
-    TcArgs a = {};
-    a.bias = bias; a.res = residual; a.out = out32; a.out16 = (__half *)out16; a.tiles = tiles;
-    a.X = X; a.Y = Y; a.Z = Z; a.cin = cin; a.cout = cout; a.act = act;
-    a.out_ld = out_ld; a.out_coff = out_coff; a.res_ld = res_ld; a.res_coff = res_coff;
-    a.tiles_y = cdiv(Y, by); a.tiles_z = cdiv(Z, TC_BZ);
-    if (!tiles) n_tiles = cdiv(X, bx) * a.tiles_y * a.tiles_z;
-    if (n_tiles <= 0) return SIS3D_OK;
-    cudaStream_t s = (cudaStream_t)stream;
-    if (wide) {
-        if (ks == 3 && by == 4) return use_cluster() ? launch_tc<64, 3, 2, 128, 4, 0, 0, 2>(tmA, tmB, a, n_tiles, s)
-                                                     : launch_tc<64, 3, 2, 128, 4>(tmA, tmB, a, n_tiles, s);
-        if (ks == 3) {
-            switch (BN) {
-                case 32: return launch_tc<32, 3, 2, 128>(tmA, tmB, a, n_tiles, s);
-                case 64: return launch_tc<64, 3, 2, 128>(tmA, tmB, a, n_tiles, s);
-                default: return launch_tc<128, 3, 2, 128>(tmA, tmB, a, n_tiles, s);
-            }
-        }
-        switch (BN) {
-            case 32: return launch_tc<32, 1, 2, 128>(tmA, tmB, a, n_tiles, s);
-            case 64: return launch_tc<64, 1, 2, 128>(tmA, tmB, a, n_tiles, s);
-            default: return launch_tc<128, 1, 2, 128>(tmA, tmB, a, n_tiles, s);
-        }
-    }
-    if (ks == 3) return BN == 32 ? launch_tc<32, 3, 2, 64>(tmA, tmB, a, n_tiles, s) : launch_tc<64, 3, 2, 64>(tmA, tmB, a, n_tiles, s);
-    return BN == 32 ? launch_tc<32, 1, 2, 64>(tmA, tmB, a, n_tiles, s) : launch_tc<64, 1, 2, 64>(tmA, tmB, a, n_tiles, s);
+    return tc_run({TC_CONV, TC_F16, in16, w16, bias, residual, res_ld, res_coff, out32, out_ld, out_coff, X, Y, Z, cin, cout, ks,
+                   tiles, n_tiles, act, stream, nullptr, 0, nullptr, 0, nullptr, (__half *)out16});
 }
 
 // brick shape the tensor-core kernel uses for a layer (so callers can build matching tile lists)
 extern "C" void sis3d_conv3d_tc_brick(int with_tile_list, int ks, int cin, int cout, int32_t *bx, int32_t *by, int32_t *bz) {
-    const int y = (with_tile_list && ks == 3 && cout == 64 && cin % 64 == 0) ? 4 : 2;
+    const int y = tc_brick_y(with_tile_list, ks, cin, cout);
     if (bx) *bx = 16 / y;
     if (by) *by = y;
     if (bz) *bz = TC_BZ;
