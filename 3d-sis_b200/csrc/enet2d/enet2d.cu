@@ -174,7 +174,7 @@ __global__ void __launch_bounds__(THREADS) enet_conv2d_kernel(const sis3d_enet_c
         }
     }
 
-    // epilogue: + bias, + residual (optionally the 2x2 max-pool of a tensor at twice the resolution, zero beyond res_c), PReLU
+    // epilogue: + bias, + residual (optionally the floor-mode 2x2 max-pool of a res_h x res_w tensor, zero beyond res_c), PReLU
 #pragma unroll
     for (int i = 0; i < TM; ++i) {
         const int64_t m = m_base + ty * TM + i;
@@ -190,9 +190,9 @@ __global__ void __launch_bounds__(THREADS) enet_conv2d_kernel(const sis3d_enet_c
             float v = acc[i][j];
             if (a.bias) v += a.bias[n];
             if (a.res && n < a.res_c) {
-                if (a.res_pool) {
-                    const int rh = 2 * a.Ho, rw = 2 * a.Wo;
-                    const float *r = a.res + (((int64_t)n_img * rh + 2 * oy) * rw + 2 * ox) * a.res_ld + n;
+                if (a.res_pool) {  // floor-mode pool: an odd res_h / res_w leaves the last row / column out
+                    const int rw = a.res_w;
+                    const float *r = a.res + (((int64_t)n_img * a.res_h + 2 * oy) * rw + 2 * ox) * a.res_ld + n;
                     v += fmaxf(fmaxf(r[0], r[a.res_ld]), fmaxf(r[(int64_t)rw * a.res_ld], r[((int64_t)rw + 1) * a.res_ld]));
                 } else {
                     v += a.res[m * a.res_ld + n];
@@ -276,11 +276,19 @@ extern "C" int sis3d_enet_pack_weight(const float *w, int cout, int cin, int kh,
 
 extern "C" int sis3d_enet_conv2d(const sis3d_enet_conv *p, void *stream) {
     if (!p || !p->in || !p->w || !p->out) return -1;
-    const sis3d_enet_conv a = *p;
+    sis3d_enet_conv a = *p;
     if (a.N <= 0 || a.H <= 0 || a.W <= 0 || a.cin <= 0 || a.cout <= 0 || a.Ho <= 0 || a.Wo <= 0 || a.kh <= 0 || a.kw <= 0 ||
         a.kh > 15 || a.kw > 15 || a.stride <= 0 || a.dil <= 0 || a.ldw < a.cout || (a.ldw & 3) || a.out_ld < a.out_coff + a.cout)
         return -1;
     if (a.res && (a.res_c <= 0 || a.res_c > a.cout || a.res_ld < a.res_c)) return -1;
+    // residual extent: [Ho][Wo], or for the pooled skip [2Ho or 2Ho + 1][2Wo or 2Wo + 1] (floor-mode 2x2/2 max-pool)
+    if (a.res_h == 0 && a.res_w == 0) {  // extent not given: the output's, or twice it for the pooled skip
+        a.res_h = (int16_t)(a.res_pool ? 2 * a.Ho : a.Ho);
+        a.res_w = (int16_t)(a.res_pool ? 2 * a.Wo : a.Wo);
+    }
+    const bool res_fits = a.res_pool ? (a.res_h == 2 * a.Ho || a.res_h == 2 * a.Ho + 1) && (a.res_w == 2 * a.Wo || a.res_w == 2 * a.Wo + 1)
+                                     : a.res_h == a.Ho && a.res_w == a.Wo;
+    if (a.res && !res_fits) return -1;
     if (((uintptr_t)a.w) & 15) return -1;
     const int64_t m_total = (int64_t)a.N * a.Ho * a.Wo;
     // narrowest N tile that covers cout (16 / 32 / 64 per grid column), vectorised gather for NHWC inputs with C_in % 4 == 0

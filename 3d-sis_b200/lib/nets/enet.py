@@ -2,12 +2,13 @@
 create_enet_for_3d :697-715; lib/nets/network.py:199-213 is where the features enter the 3-D network).
 
 `Network` builds one when cfg.USE_IMAGES and not cfg.USE_IMAGES_GT, from the `image_enet_fixed.*` / `image_enet_trainable.*`
-entries of its state_dict (same names as the reference), so raw images [n,3,256,328] are a valid input of the hot path.  The
-host side (lib/nets/enet_program.py: BatchNorm folding into a flat conv program) is checked on the CPU against the unmodified
-reference; the kernels against tests/golden/enet_encoder.npz on the GPU (tests/test_gpu_enet.py).
+entries of its state_dict (same names as the reference), so raw images [n,3,H,W] (even H and W; cfg.IMAGE_SHAPE, 256x328 by
+default) are a valid input of the hot path.  The host side (lib/nets/enet_program.py: BatchNorm folding into a flat conv
+program) is checked on the CPU against the unmodified reference; the kernels against tests/golden/enet_encoder.npz on the
+GPU (tests/test_gpu_enet.py) and launch by launch against fp64 (tests/test_gpu_enet_stage.py).
 
 Every bottleneck is three (asymmetric: four) launches of one fp32 implicit-GEMM kernel with bias / residual / PReLU fused in
-the epilogue; the down-sampling skip (2x2 max-pool + zero channel padding) is read inside the last conv's epilogue."""
+the epilogue; the down-sampling skip (floor-mode 2x2 max-pool + zero channel padding) is read inside the last conv's epilogue."""
 from __future__ import annotations
 
 import ctypes as C
@@ -23,7 +24,8 @@ class _Conv(C.Structure):
                 ("N", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("cin", C.c_int32), ("Ho", C.c_int32), ("Wo", C.c_int32),
                 ("cout", C.c_int32), ("ldw", C.c_int32), ("kh", C.c_int32), ("kw", C.c_int32), ("stride", C.c_int32),
                 ("pad_y", C.c_int32), ("pad_x", C.c_int32), ("dil", C.c_int32), ("out_ld", C.c_int32), ("out_coff", C.c_int32),
-                ("res_ld", C.c_int32), ("res_c", C.c_int32), ("res_pool", C.c_int32), ("reserved", C.c_int32)]
+                ("res_ld", C.c_int32), ("res_c", C.c_int32), ("res_pool", C.c_int32), ("res_h", C.c_int16),
+                ("res_w", C.c_int16)]
 
 
 class EnetEncoder:
@@ -84,11 +86,19 @@ class EnetEncoder:
         a.N, a.H, a.W, a.cin, a.Ho, a.Wo, a.cout, a.ldw = n, h, w, op["cin"], ho, wo, op["cout"], op["w"].shape[1]
         a.kh, a.kw, a.stride, a.pad_y, a.pad_x, a.dil = op["kh"], op["kw"], op["stride"], op["pad"][0], op["pad"][1], op["dil"]
         a.out_ld, a.out_coff, a.res_ld, a.res_c, a.res_pool = out_ld, out_coff, res_ld, res_c, res_pool
+        if res is not None:
+            a.res_h, a.res_w = res.shape[1], res.shape[2]  # the pooled skip's input may have an odd height / width
         self._check(self.lib.sis3d_enet_conv2d(C.byref(a), self._stream()))
         return ho, wo
 
     def __call__(self, images):
         """images: float32 CUDA [n,3,H,W] (normalised RGB) -> features [n,128,H/8,W/8] (NCHW, as network.py:199-213 expects)."""
+        if images.dim() == 4 and max(images.shape[2:]) > 65534:  # the residual extents are int16 in sis3d_enet_conv
+            raise ValueError(f"ENet encoder: images up to 65534 x 65534 pixels, got {tuple(images.shape)}")
+        if images.dim() != 4 or images.shape[1] != 3 or images.shape[2] % 2 or images.shape[3] % 2:
+            # the initial block concatenates a 3x3/s2 conv (ceil(H/2) rows) with a 2x2/s2 max-pool (floor(H/2) rows): the
+            # reference cannot run an odd height or width, and here the conv would write past the pooled half's rows
+            raise ValueError(f"ENet encoder: images must be [n, 3, H, W] with even H and W, got {tuple(images.shape)}")
         x_img = images.to(self.dev, torch.float32).contiguous()
         n, _, H, W = x_img.shape
         ops = iter(self.ops)

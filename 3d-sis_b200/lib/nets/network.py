@@ -653,7 +653,10 @@ class Network(nn.Module):
             if self.__dict__.get("_enet") is None:
                 raise S.Sis3dError("USE_IMAGES_GT=False but the 2-D ENet encoder was not declared (init_modules with this cfg)")
             tok = self._rec("enet_encoder")
-            feats = self._enet(feats)
+            try:
+                feats = self._enet(feats)
+            except ValueError as e:  # an input shape the encoder refuses, before anything is launched
+                raise S.Sis3dError(str(e)) from None
             self._rec_end(tok)
         n = feats.shape[0]
         if fused is None:

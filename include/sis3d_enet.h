@@ -24,8 +24,9 @@ typedef struct sis3d_enet_conv {
     int32_t N, H, W, cin, Ho, Wo, cout, ldw;
     int32_t kh, kw, stride, pad_y, pad_x, dil;
     int32_t out_ld, out_coff;
-    int32_t res_ld, res_c, res_pool;       /* res_pool = 1: the residual is the 2x2/2 max-pool of a [N][2Ho][2Wo] tensor */
-    int32_t reserved;
+    int32_t res_ld, res_c, res_pool;       /* res_pool = 1: the residual is the floor-mode 2x2/2 max-pool of the tensor */
+    int16_t res_h, res_w;                  /* residual extent: Ho x Wo, or with res_pool (2Ho | 2Ho + 1) x (2Wo | 2Wo + 1);
+                                              0 (both): Ho x Wo, with res_pool 2Ho x 2Wo (the layout before these fields) */
 } sis3d_enet_conv;
 
 /* weights [cout][cin][kh][kw] -> [kh*kw*cin][ldw] (ldw = cout rounded up to 4, zero padded) */

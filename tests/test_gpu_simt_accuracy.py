@@ -624,7 +624,8 @@ def enet_inst(N, Ho, Wo, cin, cout, nchw):
 
 
 def enet(N, H, W, cin, cout, k, *, stride=1, dil=1, nchw=False, bias=True, slope=True, res=None, res_c=None, coff=0,
-         graph=False, emu=True):
+         res_odd=(0, 0), graph=False, emu=True):
+    """res_odd: extra (rows, columns) of a pooled residual, whose floor-mode 2x2 max-pool leaves them out."""
     kh, kw = k
     py, px = (kh - 1) // 2 * dil, (kw - 1) // 2 * dil
     Ho, Wo = (H + 2 * py - dil * (kh - 1) - 1) // stride + 1, (W + 2 * px - dil * (kw - 1) - 1) // stride + 1
@@ -633,9 +634,10 @@ def enet(N, H, W, cin, cout, k, *, stride=1, dil=1, nchw=False, bias=True, slope
     rid = "-".join(str(v) for v in ("enet", inst[19:-1].replace(",", "_"), f"n{N}", f"{H}x{W}", f"{cin}to{cout}", f"k{kh}x{kw}",
                                      f"s{stride}" if stride > 1 else "", f"d{dil}" if dil > 1 else "", "nchw" if nchw else "",
                                      res or "", f"resc{res_c}" if res and res_c < cout else "", f"coff{coff}" if coff else "",
+                                     "odd{}x{}".format(*res_odd) if any(res_odd) else "",
                                      "" if slope else "noprelu") if v != "")
     return dict(fam="enet", id=rid, N=N, H=H, W=W, cin=cin, cout=cout, kh=kh, kw=kw, stride=stride, dil=dil, py=py, px=px,
-                Ho=Ho, Wo=Wo, nchw=nchw, bias=bias, slope=slope, res=res, res_c=res_c, coff=coff, graph=graph, emu=emu,
+                Ho=Ho, Wo=Wo, nchw=nchw, bias=bias, slope=slope, res=res, res_c=res_c, coff=coff, res_odd=res_odd, graph=graph, emu=emu,
                 kernels=[inst])
 
 
@@ -646,7 +648,24 @@ class EnetConv(C.Structure):
                 ("N", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("cin", C.c_int32), ("Ho", C.c_int32), ("Wo", C.c_int32),
                 ("cout", C.c_int32), ("ldw", C.c_int32), ("kh", C.c_int32), ("kw", C.c_int32), ("stride", C.c_int32),
                 ("pad_y", C.c_int32), ("pad_x", C.c_int32), ("dil", C.c_int32), ("out_ld", C.c_int32), ("out_coff", C.c_int32),
-                ("res_ld", C.c_int32), ("res_c", C.c_int32), ("res_pool", C.c_int32), ("reserved", C.c_int32)]
+                ("res_ld", C.c_int32), ("res_c", C.c_int32), ("res_pool", C.c_int32), ("res_h", C.c_int16),
+                ("res_w", C.c_int16)]
+
+
+def enet_conv_accuracy(got, acc, absum, K, epi, slope=None, mutants=None, operand_err=0.0, what="enet conv"):
+    """Assert got == prelu(acc + epi, slope) for one sis3d_enet_conv2d output within the bound of its fmaf chain,
+    gamma_(K+2) (absum + |epi|) (+ operand_err: the caller's own rounding of the operands, e.g. BatchNorm folded into the
+    weights in fp32), carried through the PReLU: times max(1, |slope|), plus one rounding of the product.  mutants: fp64
+    models (name -> pre-activation output, or (pre-activation output, slope) for a model with another PReLU slope), each
+    must miss the bound by POWER somewhere.  Returns (max err / bound, smallest model max err / bound)."""
+    pre_bound = gamma(K + 2) * (absum + epi.abs()) + operand_err
+    ref = acc + epi
+    mutants = {n: v if isinstance(v, tuple) else (v, slope) for n, v in (mutants or {}).items()}
+    if slope is None:
+        return _check(got, ref, pre_bound, {n: v for n, (v, _) in mutants.items()}, 0, what)
+    pr = lambda v, s: torch.where(v >= 0, v, v * s)
+    bound = pre_bound * slope.abs().clamp(min=1.0) + U * pr(ref, slope).abs()
+    return _check(got, pr(ref, slope), bound, {n: pr(v, s) for n, (v, s) in mutants.items()}, 0, what)
 
 
 class EnetCase:
@@ -660,7 +679,7 @@ class EnetCase:
         self.res = None
         if r["res"]:
             f = 2 if r["res"] == "pool" else 1
-            self.res = torch.randn(r["N"], f * r["Ho"], f * r["Wo"], r["res_c"], generator=g)
+            self.res = torch.randn(r["N"], f * r["Ho"] + r["res_odd"][0], f * r["Wo"] + r["res_odd"][1], r["res_c"], generator=g)
         self.m = r["N"] * r["Ho"] * r["Wo"]
         self.out_ld = r["coff"] + r["cout"] + 4
         self.res_ld = r["res_c"] + 4
@@ -687,7 +706,8 @@ class EnetCase:
         st = (cin * H * W, W, 1, H * W) if r["nchw"] else (H * W * cin, W * cin, cin, 1)
         a = EnetConv(P(o["x"]), *st, P(o["wp"]), P(o["b"]), P(o["slope"]), P(o["res"]), P(outs["out"]), r["N"], H, W, cin,
                      r["Ho"], r["Wo"], r["cout"], o["wp"].shape[1], r["kh"], r["kw"], r["stride"], r["py"], r["px"], r["dil"],
-                     self.out_ld, r["coff"], self.res_ld, r["res_c"], 1 if r["res"] == "pool" else 0, 0)
+                     self.out_ld, r["coff"], self.res_ld, r["res_c"], 1 if r["res"] == "pool" else 0,
+                     *(self.res.shape[1:3] if self.res is not None else (0, 0)))
         dev.check(dev.lib2d.sis3d_enet_conv2d(C.byref(a), dev.stream()), "sis3d_enet_conv2d")
 
     def check_layout(self, outs):
@@ -718,28 +738,23 @@ class EnetCase:
             full[:, :r["res_c"]] = rr.reshape(-1, r["res_c"])
             return full
 
-        res, top_left = torch.zeros_like(acc), None
+        res, pool_models = torch.zeros_like(acc), {}
         if self.res is not None:
             rr = self.res.to(DEV).double()
             if r["res"] == "pool":
-                top_left = residual(rr[:, ::2, ::2])
-                rr = F.max_pool2d(rr.permute(0, 3, 1, 2), 2).permute(0, 2, 3, 1)
+                pool = lambda t: F.max_pool2d(t.permute(0, 3, 1, 2), 2).permute(0, 2, 3, 1)
+                pool_models["res_pool_top_left"] = residual(rr[:, :2 * r["Ho"]:2, :2 * r["Wo"]:2])
+                if any(r["res_odd"]):  # the residual addressed as if it were [N][2Ho][2Wo]
+                    pool_models["res_pool_even_extent"] = residual(pool(rr.reshape(-1)[:self.m * 4 * r["res_c"]].reshape(
+                        r["N"], 2 * r["Ho"], 2 * r["Wo"], r["res_c"])))
+                rr = pool(rr)
             res = residual(rr)
         epi = bias + res
-        pre_bound = gamma(K + 2) * (absum + epi.abs())
         mut = {n: v + epi for n, v in mut.items()}
-        if top_left is not None:
-            mut["res_pool_top_left"] = acc + bias + top_left
-        ref = acc + epi
-        if self.slope is not None:
-            s = self.slope.to(DEV).double()
-            pr = lambda v: torch.where(v >= 0, v, v * s)
-            bound = pre_bound * torch.clamp(s, min=1.0) + U * pr(ref).abs()
-            ref, mut = pr(ref), {n: pr(v) for n, v in mut.items()}
-        else:
-            bound = pre_bound
+        mut.update({n: acc + bias + v for n, v in pool_models.items()})
         got = outs["out"][:self.m, r["coff"]:r["coff"] + cout]
-        return _check(got, ref, bound, mut, 0, r["id"])
+        slope = self.slope.to(DEV).double() if self.slope is not None else None
+        return enet_conv_accuracy(got, acc, absum, K, epi, slope, mut, what=r["id"])
 
 
 ENET_ROWS = [
@@ -755,7 +770,8 @@ ENET_ROWS = [
     enet(2, 19, 25, 64, 128, (3, 3), dil=8, res="pool", res_c=96),                  # two N blocks, K = 576
     enet(2, 40, 41, 65, 64, (3, 3), dil=16, nchw=True),                             # <64, nchw, 4>, K = 585
     enet(3, 24, 33, 32, 32, (3, 3), stride=2, res="pool"),
-]
+    enet(3, 15, 21, 64, 128, (2, 2), stride=2, res="pool", res_c=64, res_odd=(1, 1)),  # ENet's down-sampling conv1 shape,
+]                                                                                          # floor-mode pool of an odd skip
 
 
 # ------------------------------------------------------------------------------------------------ exact kernels
