@@ -35,11 +35,18 @@ class Base_Backbone(Network):
 
 
 class ScanNet_Backbone(Base_Backbone):
-    """reference: backbones.py:171-231."""
+    """reference: backbones.py:171-231.  With ONLY_IMAGES the program has no geometry1: the 128-channel colour stack is level
+    1 by itself (backbones.py:99-101, 174-176, 186)."""
 
     def _program(self):
         if cfg.ONLY_IMAGES:
-            raise NotImplementedError("ONLY_IMAGES is not used by the released configs")
+            if not cfg.USE_IMAGES:
+                raise NotImplementedError("ScanNet_Backbone with ONLY_IMAGES and USE_IMAGES=False: the reference builds a "
+                                          "0-channel geometry1 and its forward fails in geometry2.0; turn USE_IMAGES on")
+            ci = int(cfg.NUM_IMAGE_CHANNELS)
+            return dict(color=[("k2s2", 0, ci, 64), ("bneck", 2, 64, 32), ("pool", 3),
+                               ("k2s2", 4, 64, 128), ("bneck", 6, 128, 32), ("pool", 7)],
+                        geometry2=[("k3", 0, 128, 128), ("bneck", 2, 128, 64), ("bneck", 3, 128, 64), ("pool", 4)])
         g, c = (64, 64) if cfg.USE_IMAGES else (128, 0)
         prog = dict(geometry1=[("k2s2", 0, 2, 32), ("bneck", 2, 32, 32), ("bneck", 3, 32, 32),
                                ("k2s2", 4, 32, g), ("bneck", 6, g, 32), ("bneck", 7, g, 32)],
@@ -55,8 +62,10 @@ class SUNCG_Backbone(Base_Backbone):
     """reference: backbones.py:118-169."""
 
     def _program(self):
-        if cfg.ONLY_IMAGES:
-            raise NotImplementedError("ONLY_IMAGES is not used by the released configs")
+        if cfg.ONLY_IMAGES and cfg.USE_IMAGES:  # without USE_IMAGES the reference ignores ONLY_IMAGES here (:124, :148-153)
+            raise NotImplementedError("SUNCG_Backbone with ONLY_IMAGES: its level 1 is the 64-channel colour output, but the "
+                                      "reference builds rpn_net_level1 and classifier.0 for 128 channels, so its first "
+                                      "level-1 RPN conv fails")
         prog = dict(geometry1=[("k2s2", 0, 2, 64), ("bneck", 2, 64, 32), ("k2s2", 3, 64, 64), ("bneck", 5, 64, 32)],
                     geometry2=[("k3", 0, 128 if cfg.USE_IMAGES else 64, 128), ("bneck", 2, 128, 64)])
         if cfg.USE_IMAGES:

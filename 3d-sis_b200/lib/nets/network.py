@@ -737,10 +737,14 @@ class Network(nn.Module):
 
     def _backbone(self, scene: Act, imageft: Act):
         """reference: backbones.py:98-113.  Concatenation is free: both producers write their slice of
-        the level-1 tensor directly (colour channels first, then geometry)."""
+        the level-1 tensor directly (colour channels first, then geometry).  A program without geometry1 (ONLY_IMAGES) is
+        image-only: the colour stack's last op writes the whole dense level 1."""
         spec = self.SPEC
         dev = scene.t.device
-        if cfg.USE_IMAGES:
+        if "geometry1" not in spec:
+            level1 = (self._run_stack(imageft[1], "color", spec["color"][1:]) if isinstance(imageft, tuple)
+                      else self._run_stack(imageft, "color", spec["color"]))
+        elif cfg.USE_IMAGES:
             d4 = tuple((d // 2) // 2 for d in scene.dims)
             level1 = Act(torch.empty(*d4, 128, dtype=torch.float32, device=dev), d4, 128)
             def colour():

@@ -131,14 +131,21 @@ def _bottleneck(prefix, inpl, planes):
 
 
 def param_shapes(net="ScanNet_Backbone", use_images=True, num_classes=19, a1=3, a2=11,
-                 pool=4, rpn_channels=256, use_mask=True):
+                 pool=4, rpn_channels=256, use_mask=True, only_images=False):
     """state_dict names -> shapes of the 3D part of the model (ENet excluded).
 
-    ScanNet: lib/nets/backbones.py:171-231; SUNCG: 118-169; heads lib/nets/network.py:35-57;
-    mask head lib/nets/backbones.py:236-253.
+    ScanNet: lib/nets/backbones.py:171-231 (only_images: ONLY_IMAGES = USE_IMAGES = True, no geometry1 and a 128-channel
+    colour stack); SUNCG: 118-169; heads lib/nets/network.py:35-57; mask head lib/nets/backbones.py:236-253.
     """
     s = []
-    if net == "ScanNet_Backbone":
+    if only_images:
+        if net != "ScanNet_Backbone" or not use_images:
+            raise ValueError("only_images: ScanNet_Backbone with use_images")
+        s += [("color.0.weight", (64, 128, 2, 2, 2))] + _bottleneck("color.2", 64, 32)
+        s += [("color.4.weight", (128, 64, 2, 2, 2))] + _bottleneck("color.6", 128, 32)
+        s += [("geometry2.0.weight", (128, 128, 3, 3, 3))]
+        s += _bottleneck("geometry2.2", 128, 64) + _bottleneck("geometry2.3", 128, 64)
+    elif net == "ScanNet_Backbone":
         gch, cch = (64, 64) if use_images else (128, 0)
         s += [("geometry1.0.weight", (32, 2, 2, 2, 2))]
         s += _bottleneck("geometry1.2", 32, 32) + _bottleneck("geometry1.3", 32, 32)
@@ -250,12 +257,13 @@ def build_case(port, c):
     return cfg, w, data, views
 
 
-def make_net(c, keep_debug=True, math="fp32", weights=None, enet=False, gt_rois=None):
+def make_net(c, keep_debug=True, math="fp32", weights=None, enet=False, gt_rois=None, only_images=False):
     """The product Network for a case: released yml config, seeded synthetic weights loaded through load_state_dict.
     enet=True: cfg.USE_IMAGES_GT=False -- the blobs carry RGB frames and the 2-D ENet encoder (seeded default init) is part
     of the forward.  gt_rois=True / False: test mode on ground-truth boxes and classes (USE_RPN = USE_CLASS = False) with
     USE_BACKBONE on / off; the weights are those of the same model without RPN and classifier heads (the ones
-    oracle/make_golden_gt_rois.py loads into the reference)."""
+    oracle/make_golden_gt_rois.py loads into the reference).  only_images=True: the image-only ScanNet backbone (ONLY_IMAGES)
+    with the weights of param_shapes(only_images=True)."""
     import os
     import torch
     from lib.utils.config import cfg, cfg_from_file, cfg_reset
@@ -264,6 +272,7 @@ def make_net(c, keep_debug=True, math="fp32", weights=None, enet=False, gt_rois=
     cfg_from_file(os.path.join(os.path.dirname(os.path.abspath(__file__)), "experiments", "cfgs", yml, "rpn_class_mask_5.yml"))
     cfg.NUM_CLASSES = 26 if c["cfgname"] == "suncg" else 19
     cfg.USE_IMAGES, cfg.USE_MASK, cfg.USE_IMAGES_GT = c["use_images"], c["use_mask"], not enet
+    cfg.ONLY_IMAGES = bool(only_images)
     if gt_rois is not None:
         cfg.USE_RPN, cfg.USE_CLASS, cfg.USE_BACKBONE = False, False, bool(gt_rois)
     from lib.nets import backbones
@@ -277,7 +286,7 @@ def make_net(c, keep_debug=True, math="fp32", weights=None, enet=False, gt_rois=
                    if not k.startswith("classifier_")}
     w = weights if weights is not None else make_weights(
         seed=0, net=cfg.NET, use_images=c["use_images"], num_classes=cfg.NUM_CLASSES, a1=cfg.NUM_ANCHORS_LEVEL1,
-        a2=cfg.NUM_ANCHORS_LEVEL2, use_mask=c["use_mask"])
+        a2=cfg.NUM_ANCHORS_LEVEL2, use_mask=c["use_mask"], only_images=only_images)
     net.load_state_dict({k: torch.from_numpy(v) for k, v in w.items()}, strict=not enet)
     net._keep_debug = keep_debug
     net.set_conv_math(math)
