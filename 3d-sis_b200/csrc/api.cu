@@ -199,6 +199,145 @@ extern "C" int sis3d_mask_stage_launch(const sis3d_mask_plan *p, const void *h_b
     return SIS3D_OK;
 }
 
+// ---- colour-aware ragged mask stage (MASK_USE_IMAGES / MASK_ONLY_IMAGES) -----------------------------------------------------
+// Buffers, in the route's operand type: A and B (64 channels) ping-pong through each stack; I (128 channels) holds the
+// gathered colour input until colour.0 has read it, then the concatenation [geometry | colour] that the two 1x1s write; A and B
+// together (128 channels) then hold combine.0's output (math 2: canvas32).  The canvas routes keep every voxel outside the
+// crops zero (the crops' padding): nothing writes there.  The 128 -> 128 combine.0 runs as two 128 -> 64 halves on the
+// 4x4x8-brick instances, the ones colour.0 and the 64 -> 64 layers use.
+extern "C" int sis3d_mask_stage_color_launch(const sis3d_mask_plan *p, const sis3d_mask_color_plan *cp, const void *h_blob,
+                                             const sis3d_mask_stage_color *a, void *stream) {
+    if (!p || !cp || !h_blob || !a || !a->scene || !a->w_color_first || !a->w_color_last || !a->tables || !a->canvas || !a->masks)
+        return SIS3D_EINVAL;
+    const bool full = !a->only_images;
+    if (full && (!a->w_geom_first || !a->w_geom_last || !a->w_combine || !a->w_combine_last)) return SIS3D_EINVAL;
+    for (int i = 0; i < 4; ++i)
+        if (!a->w_color_mid[i] || (full && !a->w_geom_mid[i])) return SIS3D_EINVAL;
+    if (a->math < 0 || a->math > 2) return SIS3D_EINVAL;
+    const int nk = p->n_kept, ncls = a->ncls;
+    if (nk <= 0) return SIS3D_OK;
+    if (a->crop_in ? nk != 1 : (!a->feats_t || !a->pix || !a->pairs || !a->n_pairs || a->n_views <= 0 || a->hw <= 0))
+        return SIS3D_EINVAL;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int64_t total = p->total_voxels;
+    const int Xc = p->canvas[0], Yc = p->canvas[1], Zc = p->canvas[2];
+    const int64_t cvox = (int64_t)Xc * Yc * Zc, vox = a->math == 0 ? total : cvox;
+    const size_t eb = a->math == 2 ? 2 : 4, need = (size_t)vox * 64 * eb * 4;
+    if (a->canvas_bytes < need) return SIS3D_EWORKSPACE;
+    if (a->math == 2 && (!a->canvas32 || a->canvas32_bytes < (size_t)cvox * (full ? 128 : 64) * 4)) return SIS3D_EWORKSPACE;
+    if (cudaMemcpyAsync(a->tables, h_blob, (size_t)cp->bytes, cudaMemcpyHostToDevice, st) != cudaSuccess) return SIS3D_ELAUNCH;
+    if (a->math && cudaMemsetAsync(a->canvas, 0, need, st) != cudaSuccess) return SIS3D_ELAUNCH;
+    char *tb = (char *)a->tables;
+    const sis3d_region *r_first = (const sis3d_region *)(tb + p->off_first), *r_last = (const sis3d_region *)(tb + p->off_last);
+    const sis3d_region *r_mid = (const sis3d_region *)(tb + p->off_rest), *r_g2c = (const sis3d_region *)(tb + cp->off_g2c);
+    const sis3d_region *r_last128 = (const sis3d_region *)(tb + cp->off_last128);
+    const int32_t *tiles = (const int32_t *)(tb + p->off_rest);
+    const int nt = p->n_tiles_tc;
+    const int64_t scene_vox = (int64_t)a->X * a->Y * a->Z;
+    char *A = (char *)a->canvas, *B = A + (size_t)vox * 64 * eb, *I = B + (size_t)vox * 64 * eb;
+    int rc;
+    // colour input
+    if (a->crop_in) {  // one crop at canvas x 0 (canvas y, z = the crop's h, l): its voxels are the first w*h*l rows, as compact
+        if (a->math == 2) {
+            if ((rc = sis3d_cast_f16(a->crop_in, 128, 0, total, 128, (uint16_t *)I, stream))) return rc;
+        } else if (cudaMemcpyAsync(I, a->crop_in, (size_t)total * 128 * 4, cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
+            return SIS3D_ELAUNCH;
+        }
+    } else if ((rc = sis3d_mask_color_gather(a->feats_t, a->pix, a->pairs, a->n_pairs, a->n_views, 128, a->hw, a->X, a->Y, a->Z,
+                                             (const int32_t *)(tb + cp->off_crops), (const int64_t *)(tb + p->off_offs), nk, total,
+                                             Yc, Zc, a->math, I, stream))) {
+        return rc;
+    }
+    // one 3x3x3 stack: first layer (scene or colour input) -> A, four 64 -> 64 layers; returns the fp32 input of its 1x1
+    auto stack = [&](bool colour, const float **x32) -> int {
+        const void *const *mid = colour ? a->w_color_mid : a->w_geom_mid;
+        if (a->math == 0) {
+            float *cur = (float *)A, *nxt = (float *)B;
+            if (colour) rc = sis3d_conv3d_ex((const float *)I, 1, (const float *)a->w_color_first, nullptr, nullptr, 0, 0, cur, nullptr,
+                                             64, 0, (const sis3d_region *)(tb + cp->off_c0), nk, p->tiles_mid, 128, 64, 3, 1, 1, 1, stream);
+            else rc = sis3d_conv3d_ex(a->scene, scene_vox, a->w_geom_first, nullptr, nullptr, 0, 0, cur, nullptr, 64, 0, r_first, nk,
+                                      p->tiles_first, 2, 64, 3, 1, 1, 1, stream);
+            if (rc) return rc;
+            for (int i = 0; i < 4; ++i) {
+                if ((rc = sis3d_conv3d_ex(cur, 1, (const float *)mid[i], nullptr, nullptr, 0, 0, nxt, nullptr, 64, 0, r_mid, nk,
+                                          p->tiles_mid, 64, 64, 3, 1, 1, 1, stream))) return rc;
+                float *t = cur; cur = nxt; nxt = t;
+            }
+            *x32 = cur;
+        } else if (a->math == 2) {
+            uint16_t *cur = (uint16_t *)A, *nxt = (uint16_t *)B;
+            if (colour) rc = sis3d_conv3d_tc_f16((const uint16_t *)I, (const uint16_t *)a->w_color_first, nullptr, nullptr, 0, 0, nullptr,
+                                                 cur, 64, 0, Xc, Yc, Zc, 128, 64, 3, tiles, nt, 1, stream);
+            else rc = sis3d_conv3d_ex(a->scene, scene_vox, a->w_geom_first, nullptr, nullptr, 0, 0, nullptr, cur, 64, 0, r_first, nk,
+                                      p->tiles_first, 2, 64, 3, 1, 1, 1, stream);
+            if (rc) return rc;
+            for (int i = 0; i < 4; ++i) {
+                const bool last3 = i == 3;
+                if ((rc = sis3d_conv3d_tc_f16(cur, (const uint16_t *)mid[i], nullptr, nullptr, 0, 0, last3 ? a->canvas32 : nullptr,
+                                              last3 ? nullptr : nxt, 64, 0, Xc, Yc, Zc, 64, 64, 3, tiles, nt, 1, stream))) return rc;
+                uint16_t *t = cur; cur = nxt; nxt = t;
+            }
+            *x32 = a->canvas32;
+        } else {
+            float *cur = (float *)A, *nxt = (float *)B;
+            if (colour) rc = sis3d_conv3d_k3_tc((const float *)I, (const float *)a->w_color_first, nullptr, nullptr, 0, 0, cur, 64, 0,
+                                                Xc, Yc, Zc, 128, 64, 3, tiles, nt, 1, stream);
+            else rc = sis3d_conv3d_ex(a->scene, scene_vox, a->w_geom_first, nullptr, nullptr, 0, 0, cur, nullptr, 64, 0, r_first, nk,
+                                      p->tiles_first, 2, 64, 3, 1, 1, 1, stream);
+            if (rc) return rc;
+            for (int i = 0; i < 4; ++i) {
+                if ((rc = sis3d_conv3d_k3_tc(cur, (const float *)mid[i], nullptr, nullptr, 0, 0, nxt, 64, 0, Xc, Yc, Zc, 64, 64, 3, tiles,
+                                             nt, 1, stream))) return rc;
+                float *t = cur; cur = nxt; nxt = t;
+            }
+            *x32 = cur;
+        }
+        return SIS3D_OK;
+    };
+    // a stack's 1x1 (64 -> 64, no ReLU) writing channels [coff, coff + 64) of the concatenation in I
+    auto to_cat = [&](const float *x32, const float *w, int coff) -> int {
+        return sis3d_conv3d_ex(x32, 1, w, nullptr, nullptr, 0, 0, a->math == 2 ? nullptr : (float *)I,
+                               a->math == 2 ? (uint16_t *)I : nullptr, 128, coff, r_g2c, nk, p->tiles_last, 64, 64, 1, 1, 0, 0, stream);
+    };
+    const float *x32 = nullptr, *head_in = nullptr;
+    if ((rc = stack(true, &x32))) return rc;
+    if (!full) {
+        if ((rc = sis3d_conv3d_ex(x32, 1, a->w_color_last, nullptr, nullptr, 0, 0, a->masks, nullptr, ncls, 0, r_last, nk, p->tiles_last,
+                                  64, ncls, 1, 1, 0, 2, stream))) return rc;
+    } else {
+        if ((rc = to_cat(x32, a->w_color_last, 64))) return rc;
+        if ((rc = stack(false, &x32))) return rc;
+        if ((rc = to_cat(x32, a->w_geom_last, 0))) return rc;
+        // combine.0: 128 -> 128 + ReLU
+        if (a->math == 0) {
+            rc = sis3d_conv3d_ex((const float *)I, 1, (const float *)a->w_combine, nullptr, nullptr, 0, 0, (float *)A, nullptr, 128, 0,
+                                 (const sis3d_region *)(tb + cp->off_c128), nk, p->tiles_mid, 128, 128, 3, 1, 1, 1, stream);
+            head_in = (const float *)A;
+        } else {
+            const size_t half = (size_t)64 * 27 * 128;  // weight rows of 64 output channels
+            for (int hh = 0; hh < 2 && !rc; ++hh) {
+                if (a->math == 2)
+                    rc = sis3d_conv3d_tc_f16((const uint16_t *)I, (const uint16_t *)a->w_combine + hh * half, nullptr, nullptr, 0, 0,
+                                             a->canvas32, nullptr, 128, 64 * hh, Xc, Yc, Zc, 128, 64, 3, tiles, nt, 1, stream);
+                else
+                    rc = sis3d_conv3d_k3_tc((const float *)I, (const float *)a->w_combine + hh * half, nullptr, nullptr, 0, 0,
+                                            (float *)A, 128, 64 * hh, Xc, Yc, Zc, 128, 64, 3, tiles, nt, 1, stream);
+            }
+            head_in = a->math == 2 ? a->canvas32 : (const float *)A;
+        }
+        if (rc) return rc;
+        if ((rc = sis3d_conv3d_ex(head_in, 1, a->w_combine_last, nullptr, nullptr, 0, 0, a->masks, nullptr, ncls, 0, r_last128, nk,
+                                  p->tiles_last, 128, ncls, 1, 1, 0, 2, stream))) return rc;
+    }
+    if (a->bits) {
+        if ((rc = sis3d_mask_select(a->masks, (const int64_t *)(tb + p->off_offs), (const int32_t *)(tb + p->off_cls), nk, ncls,
+                                    total, a->thresh, nullptr, a->bits, stream))) return rc;
+        if (a->bits_host && cudaMemcpyAsync(a->bits_host, a->bits, (size_t)total, cudaMemcpyDeviceToHost, st) != cudaSuccess)
+            return SIS3D_ELAUNCH;
+    }
+    return SIS3D_OK;
+}
+
 // thin async-copy entry point for hosts that stage their own pinned buffers (kind: 1 H2D, 2 D2H, 3 D2D)
 extern "C" int sis3d_memcpy_async(void *dst, const void *src, size_t bytes, int kind, void *stream) {
     if (!dst || !src) return SIS3D_EINVAL;

@@ -56,6 +56,24 @@ class MaskStage(C.Structure):
                 ("bits_host", C.c_void_p), ("thresh", C.c_float), ("reserved2", C.c_int32)]
 
 
+class MaskColorPlan(C.Structure):
+    """struct sis3d_mask_color_plan (include/sis3d.h)."""
+    _fields_ = [("off_crops", C.c_int64), ("off_g2c", C.c_int64), ("off_last128", C.c_int64), ("off_c0", C.c_int64),
+                ("off_c128", C.c_int64), ("bytes", C.c_int64)]
+
+
+class MaskStageColor(C.Structure):
+    """struct sis3d_mask_stage_color (include/sis3d.h)."""
+    _fields_ = [("scene", C.c_void_p), ("X", C.c_int32), ("Y", C.c_int32), ("Z", C.c_int32), ("ncls", C.c_int32),
+                ("math", C.c_int32), ("only_images", C.c_int32), ("w_geom_first", C.c_void_p), ("w_geom_last", C.c_void_p),
+                ("w_geom_mid", C.c_void_p * 4), ("w_color_first", C.c_void_p), ("w_color_mid", C.c_void_p * 4),
+                ("w_color_last", C.c_void_p), ("w_combine", C.c_void_p), ("w_combine_last", C.c_void_p), ("feats_t", C.c_void_p),
+                ("pix", C.c_void_p), ("pairs", C.c_void_p), ("n_pairs", C.c_void_p), ("n_views", C.c_int32), ("hw", C.c_int32),
+                ("crop_in", C.c_void_p), ("tables", C.c_void_p), ("canvas", C.c_void_p), ("canvas_bytes", C.c_size_t),
+                ("canvas32", C.c_void_p), ("canvas32_bytes", C.c_size_t), ("masks", C.c_void_p), ("bits", C.c_void_p),
+                ("bits_host", C.c_void_p), ("thresh", C.c_float), ("reserved", C.c_int32)]
+
+
 REGION_BYTES = C.sizeof(Region)
 TILE_M = 64
 
@@ -69,6 +87,7 @@ SYMBOLS = ["sis3d_strerror", "sis3d_version", "sis3d_launch_count", "sis3d_nms_w
            "sis3d_backproject_conv_k2s2_ex", "sis3d_linear_workspace_bytes", "sis3d_linear", "sis3d_linear_tc_supported", "sis3d_linear_tc_workspace_bytes", "sis3d_linear_tc", "sis3d_mlp_tail", "sis3d_pack_conv_weight_tc", "sis3d_conv3d_k3_tc_supported", "sis3d_conv3d_tc_brick", "sis3d_conv3d_k3_tc",
            "sis3d_conv3d_k3_tc_fused_supported", "sis3d_conv3d_k3_tc_fused",
            "sis3d_rpn_workspace_bytes", "sis3d_rpn_proposals", "sis3d_detect_decode", "sis3d_mask_plan_build", "sis3d_mask_stage_launch", "sis3d_memcpy_async",
+           "sis3d_mask_color_plan_build", "sis3d_mask_color_gather", "sis3d_mask_color_feats_t", "sis3d_mask_stage_color_launch",
            "sis3d_mask_select", "sis3d_pack_conv_weight_tc_x3", "sis3d_conv3d_k3_tc_x3", "sis3d_conv3d_k3_tc_fused_x3",
            "sis3d_linear_tc_x3", "sis3d_pack_conv_weight_tc_h3", "sis3d_conv3d_k3_tc_h3", "sis3d_conv3d_k3_tc_fused_h3",
            "sis3d_linear_tc_h3", "sis3d_chunk_decode", "sis3d_conv3d_k1_tc_h3_split", "sis3d_conv3d_k3_tc_fused_h3_split", "sis3d_mask_overlap",

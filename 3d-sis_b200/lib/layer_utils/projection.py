@@ -130,12 +130,14 @@ class ProjectionHelper:
         return lin3d, lin2d
 
 
-def backproject(feats, pix, pairs, n_pairs, volume_dims, img_w, img_h):
-    """feats [n,C,h,w] cuda -> VC volume [X,Y,Z,C] = max over paired views of (covered ? f : 0)."""
+def backproject(feats, pix, pairs, n_pairs, volume_dims, img_w, img_h, feats_t=None):
+    """feats [n,C,h,w] cuda -> VC volume [X,Y,Z,C] = max over paired views of (covered ? f : 0).  feats_t: where the
+    channels-last copy of the features [n,h*w,C] goes (a new tensor when None)."""
     X, Y, Z = (int(v) for v in volume_dims)
     n, Cn = feats.shape[0], feats.shape[1]
     feats = feats.contiguous()
-    feats_t = torch.empty(n, img_w * img_h, Cn, dtype=torch.float32, device=feats.device)
+    if feats_t is None:
+        feats_t = torch.empty(n, img_w * img_h, Cn, dtype=torch.float32, device=feats.device)
     vol = torch.empty(X, Y, Z, Cn, dtype=torch.float32, device=feats.device)
     S.check(S.lib.sis3d_backproject_max(S.ptr(feats), S.ptr(feats_t), S.ptr(pix), S.ptr(pairs), S.ptr(n_pairs), n, Cn,
                                         img_w, img_h, X, Y, Z, S.ptr(vol), S.stream()), "backproject_max")

@@ -75,34 +75,62 @@ class SUNCG_Backbone(Base_Backbone):
 
 
 class MaskBackbone(nn.Module):
-    """Per-RoI mask head: 5 x (conv3x3x3 -> ReLU) + 1x1 -> sigmoid, no biases (reference:
-    backbones.py:236-287).  Parameters live here (state_dict keys mask_backbone.geometry.N.weight); the
-    kernels are launched through the owning Network so the packed weights are shared."""
+    """Per-RoI mask head: 5 x (conv3x3x3 -> ReLU) + 1x1 -> sigmoid, no biases (reference: backbones.py:236-287).  Parameters
+    live here (state_dict keys mask_backbone.geometry.N.weight); the kernels are launched through the owning Network so the
+    packed weights are shared.  With MASK_USE_IMAGES the geometry stack ends in a 64 -> 64 1x1, a colour stack (128 -> 64, four
+    64 -> 64, 1x1) runs on the crop of the back-projected image features, and `combine` (128 -> 128 + ReLU, 1x1 -> classes)
+    runs on [geometry | colour]; with MASK_ONLY_IMAGES the colour stack alone makes the masks (its 1x1 -> classes), and
+    geometry and combine are declared but not run.  The switches are read once, here: a net built colour-aware stays so."""
+
+    @staticmethod
+    def refuse_unrunnable():
+        """The two mask-switch combinations the reference cannot run, refused before any parameter is declared."""
+        if cfg.MASK_USE_IMAGES and not cfg.USE_IMAGES:
+            raise NotImplementedError("MASK_USE_IMAGES with USE_IMAGES=False: the reference has no image features to crop "
+                                      "(self.color(None) fails); turn USE_IMAGES on")
+        if cfg.MASK_ONLY_IMAGES and not cfg.MASK_USE_IMAGES:
+            raise NotImplementedError("MASK_ONLY_IMAGES without MASK_USE_IMAGES: the reference builds no colour stack and its "
+                                      "forward fails with an AttributeError; turn MASK_USE_IMAGES on too")
 
     def __init__(self):
         super().__init__()
-        if cfg.MASK_USE_IMAGES or cfg.MASK_ONLY_IMAGES:
-            raise NotImplementedError("MASK_USE_IMAGES is off in the released configs (config.py:100)")
+        self.refuse_unrunnable()
         from lib.nets.network import _declare
-        cin = 2
-        for i in (0, 2, 4, 6, 8):
-            _declare(self, f"geometry.{i}.weight", (64, cin, 3, 3, 3), cin * 27)
-            cin = 64
-        _declare(self, "geometry.10.weight", (int(cfg.NUM_CLASSES), 64, 1, 1, 1), 64)
+        nc = int(cfg.NUM_CLASSES)
+        self.colour, self.only_images = bool(cfg.MASK_USE_IMAGES), bool(cfg.MASK_ONLY_IMAGES)
+        stacks = [("geometry", 2, 64 if self.colour else nc)]
+        if self.colour:
+            stacks.append(("color", 128, nc if self.only_images else 64))
+        for stack, cin, last in stacks:
+            for i in (0, 2, 4, 6, 8):
+                _declare(self, f"{stack}.{i}.weight", (64, cin, 3, 3, 3), cin * 27)
+                cin = 64
+            _declare(self, f"{stack}.10.weight", (last, 64, 1, 1, 1), 64)
+        if self.colour:
+            _declare(self, "combine.0.weight", (128, 128, 3, 3, 3), 128 * 27)
+            _declare(self, "combine.2.weight", (nc, 128, 1, 1, 1), 128)
         self._owner = None
 
     def forward(self, scene, imageft=None):
-        """scene [1,2,w,h,l] crop (NCDHW) -> sigmoid mask [1,num_classes,w,h,l]."""
+        """scene [1,2,w,h,l] crop (NCDHW), imageft its [1,128,w,h,l] crop of the back-projected image features (colour-aware
+        heads) -> sigmoid mask [1,num_classes,w,h,l]."""
         net = self._owner() if self._owner is not None else None
         if net is None:
             raise S.Sis3dError("mask_backbone is launched through its owning Network (which is gone)")
         net._ensure_packed()
         if scene.shape[0] != 1:
             raise S.Sis3dError("mask_backbone: batch size 1")
-        scene = scene.to(next(net.parameters()).device, torch.float32).contiguous()
+        dev = next(net.parameters()).device
+        scene = scene.to(dev, torch.float32).contiguous()
         w, h, l = (int(v) for v in scene.shape[2:])
+        color = None
+        if self.colour:
+            if imageft is None or tuple(imageft.shape) != (1, 128, w, h, l):
+                raise S.Sis3dError(f"mask_backbone: a colour-aware head takes the [1, 128, {w}, {h}, {l}] image-feature crop, got "
+                                   f"{None if imageft is None else tuple(imageft.shape)}")
+            color = dict(crop_in=imageft[0].to(dev, torch.float32).permute(1, 2, 3, 0).contiguous())
         det = torch.zeros(1, 16)
         det[0, 8] = 1.0
         det[0, 12:15] = torch.tensor([w, h, l], dtype=torch.float32)
-        masks = net._mask_branch(scene, det.numpy(), 1)
+        masks = net._mask_branch(scene, det.numpy(), 1, color=color)
         return masks[0].contiguous()

@@ -215,6 +215,9 @@ class Network(nn.Module):
 
     def init_modules(self):
         """Declare every parameter of the 3D model (reference: network.py:35-64)."""
+        if cfg.USE_MASK:
+            from lib.nets.backbones import MaskBackbone
+            MaskBackbone.refuse_unrunnable()
         self._init_backbone_classifier()
         if cfg.USE_RPN:
             for lvl in (1, 2, 3):
@@ -640,8 +643,9 @@ class Network(nn.Module):
             self._const_cache[key] = v
         return v
 
-    def _backproject(self, blobs, killing_inds, dims, dev, fused=None):
-        """Views -> VC feature volume (reference: trainval.py:797-820 + network.py:194-239)."""
+    def _view_maps(self, blobs, killing_inds, dims, dev, fused=None):
+        """Views -> (features [n,C,h,w], voxel->pixel maps, (feature, map) pairs, pair count): the inputs of every
+        back-projection (reference: trainval.py:797-820 + network.py:194-223)."""
         w, h = int(cfg.DEPTH_SHAPE[0]), int(cfg.DEPTH_SHAPE[1])
         if fused is not None:
             feats = fused["feats"]
@@ -685,6 +689,18 @@ class Network(nn.Module):
             n_pairs = torch.empty(1, dtype=torch.int32, device=dev)
             S.check(S.lib.sis3d_backproject_pairs(S.ptr(counts), n, S.ptr(pairs), S.ptr(n_pairs), S.stream()), "pairs")
             self._proj_counts = counts
+        return feats, pix, pairs, n_pairs
+
+    def _backproject(self, blobs, killing_inds, dims, dev, fused=None):
+        """Views -> VC feature volume (reference: trainval.py:797-820 + network.py:194-239).  A colour-aware mask head gathers
+        its crops from the same maps later: for it they and the channels-last features are left in self._color_src."""
+        w, h = int(cfg.DEPTH_SHAPE[0]), int(cfg.DEPTH_SHAPE[1])
+        feats, pix, pairs, n_pairs = self._view_maps(blobs, killing_inds, dims, dev, fused)
+        feats = feats.contiguous()
+        feats_t = torch.empty(feats.shape[0], w * h, feats.shape[1], dtype=torch.float32, device=dev)
+        if self._mask_colour():
+            self.__dict__["_color_src"] = dict(feats_t=feats_t, pix=pix, pairs=pairs, n_pairs=n_pairs, n_views=feats.shape[0],
+                                               hw=w * h)
         first = self.SPEC["color"][0]
         if (self._sparse_color and not self._keep_debug and first[0] == "k2s2" and feats.shape[1] % 16 == 0
                 and first[3] in (32, 64)):
@@ -694,8 +710,6 @@ class Network(nn.Module):
             out = Act(torch.empty(*od, cout, dtype=torch.float32, device=dev), od, cout)
             if self._math == "fp16":
                 out.h = torch.empty(*od, cout, dtype=torch.float16, device=dev)
-            feats = feats.contiguous()
-            feats_t = torch.empty(feats.shape[0], w * h, feats.shape[1], dtype=torch.float32, device=dev)
             nbytes = int(S.lib.sis3d_backproject_conv_k2s2_workspace_bytes(*dims, cout))
             ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
             tok = self._rec("backproject_conv_k2s2")
@@ -707,7 +721,7 @@ class Network(nn.Module):
             self._rec_end(tok)
             return ("color0", out)
         tok = self._rec("backproject_max")
-        vol = proj.backproject(feats, pix, pairs, n_pairs, dims, w, h)
+        vol = proj.backproject(feats, pix, pairs, n_pairs, dims, w, h, feats_t=feats_t)
         self._rec_end(tok)
         return Act(vol, dims, feats.shape[1])
 
@@ -834,30 +848,48 @@ class Network(nn.Module):
             self._predictions["pool5"] = pool5
         return cls_score.t.view(R, -1), bbox_pred.t.view(R, -1)
 
-    def _mask_branch(self, scene_ncdhw, det_host, n, extras=None):
+    def _mask_colour(self):
+        """The mask head runs the colour stack (built with MASK_USE_IMAGES)."""
+        mb = self._modules.get("mask_backbone")
+        return mb is not None and mb.colour
+
+    def _mask_plan(self, det_host, n, X, Y, Z, ncls, canvas, dev, colour):
+        """The planner's tables (and the colour stage's, appended) in the pinned staging blob: (plan, color plan, blob)."""
+        plan, cplan = S.MaskPlan(), S.MaskColorPlan()
+        cap = self._arena["mask_tables_host"].numel() if "mask_tables_host" in self._arena else 1 << 18
+        while True:
+            stage = self._ws("mask_tables_host", cap, torch.uint8, dev, pinned=True)
+            blob, size = C.c_void_p(stage.data_ptr()), C.c_size_t(stage.numel())
+            rc = S.lib.sis3d_mask_plan_build(C.c_void_p(det_host.ctypes.data), n, X, Y, Z, ncls, 1 if canvas else 0, blob, size,
+                                             C.byref(plan))
+            if rc == 0 and colour:
+                rc = S.lib.sis3d_mask_color_plan_build(C.c_void_p(det_host.ctypes.data), n, C.byref(plan), blob, size, C.byref(cplan))
+                if rc == -3:
+                    cap = int(cplan.bytes) * 2
+                    continue
+            if rc == -3:  # SIS3D_EWORKSPACE: grow the pinned staging buffer and retry
+                cap = int(plan.bytes) * 2
+                continue
+            S.check(rc, "mask_plan_build")
+            return plan, cplan, stage
+
+    def _mask_branch(self, scene_ncdhw, det_host, n, extras=None, color=None):
         """Ragged per-RoI mask head (reference: network.py:283-317).  All kept crops are packed along x on
         one zeroed canvas [sum(w_j + 1), max h, max l, 64] (one zero slab between crops = the crop-border
         zero padding), so each of the six layers is ONE launch: layer 1 (C_in = 2, windowed NCDHW scene) and
         the 1x1 head on the fp32 CUDA-core kernel, the four 64->64 3x3x3 layers on the wgmma kernel driven
         by an explicit list of 4x4x8 bricks.  The tables come from the native planner (sis3d_mask_plan_build)
-        and travel in ONE pinned H2D copy; all buffers come from a grow-only arena."""
+        and travel in ONE pinned H2D copy; all buffers come from a grow-only arena.  A colour-aware head runs
+        _mask_branch_color on `color` (the static stage's colour sources, or crop_in: a dense crop of the image features)."""
+        if self._mask_colour():
+            return self._mask_branch_color(scene_ncdhw, det_host, n, extras, color)
         dev = scene_ncdhw.device
         X, Y, Z = (int(v) for v in scene_ncdhw.shape[2:])
         ncls = self._layers["mask_backbone.geometry.10"][1]
         math = self.MASK_ROUTES.index(self._mask_math)  # route: 0 CUDA-core, 1 TF32, 2 fp16 operands (the 64->64 layers)
         W = self._packs
         det_host = np.ascontiguousarray(det_host[:n], dtype=np.float32)
-        plan = S.MaskPlan()
-        cap = self._arena["mask_tables_host"].numel() if "mask_tables_host" in self._arena else 1 << 18
-        while True:
-            stage = self._ws("mask_tables_host", cap, torch.uint8, dev, pinned=True)
-            rc = S.lib.sis3d_mask_plan_build(C.c_void_p(det_host.ctypes.data), n, X, Y, Z, ncls, 1 if math else 0,
-                                             C.c_void_p(stage.data_ptr()), C.c_size_t(stage.numel()), C.byref(plan))
-            if rc == -3:  # SIS3D_EWORKSPACE: grow the pinned staging buffer and retry
-                cap = int(plan.bytes) * 2
-                continue
-            S.check(rc, "mask_plan_build")
-            break
+        plan, _, stage = self._mask_plan(det_host, n, X, Y, Z, ncls, math != 0, dev, False)
         nk = int(plan.n_kept)
         if nk == 0:
             return []
@@ -891,6 +923,67 @@ class Network(nn.Module):
         self._rec_end(tok)
         return _MaskList(outb, offs, sizes, ncls)
 
+    def _mask_branch_color(self, scene_ncdhw, det_host, n, extras, color):
+        """The colour-aware ragged mask stage (MASK_USE_IMAGES / MASK_ONLY_IMAGES; reference: backbones.py:236-287): the
+        layout of _mask_branch with a 128-channel colour input per crop, gathered on the device from the view maps and
+        features in `color` (or copied from color['crop_in']), and ONE call of sis3d_mask_stage_color_launch."""
+        if color is None:
+            raise S.Sis3dError("the colour-aware mask head needs the scene's image features (USE_IMAGES inputs)")
+        dev = scene_ncdhw.device
+        X, Y, Z = (int(v) for v in scene_ncdhw.shape[2:])
+        mb, pre = self.mask_backbone, "mask_backbone."
+        only = mb.only_images
+        ncls = self._layers[pre + ("color.10" if only else "combine.2")][1]
+        math = self.MASK_ROUTES.index(self._mask_math)
+        W, F = self._packs, self._mask_math
+        det_host = np.ascontiguousarray(det_host[:n], dtype=np.float32)
+        plan, cplan, stage = self._mask_plan(det_host, n, X, Y, Z, ncls, math != 0, dev, True)
+        nk = int(plan.n_kept)
+        if nk == 0:
+            return []
+        total = int(plan.total_voxels)
+        host = stage.numpy()
+        offs = host[plan.off_offs:plan.off_offs + 8 * (nk + 1)].view(np.int64).copy()
+        sizes = host[plan.off_sizes:plan.off_sizes + 12 * nk].view(np.int32).reshape(nk, 3).copy()
+        cvox = int(plan.canvas[0]) * int(plan.canvas[1]) * int(plan.canvas[2])
+        a = S.MaskStageColor()
+        a.scene, a.X, a.Y, a.Z, a.ncls, a.math, a.only_images = scene_ncdhw.data_ptr(), X, Y, Z, ncls, math, int(only)
+        a.w_color_first = W[F][pre + "color.0"].data_ptr()
+        a.w_color_last = W["fp32"][pre + "color.10"].data_ptr()
+        for i, idx in enumerate((2, 4, 6, 8)):
+            a.w_color_mid[i] = W[F][f"{pre}color.{idx}"].data_ptr()
+        if not only:
+            a.w_geom_first = W["fp32"][pre + "geometry.0"].data_ptr()
+            a.w_geom_last = W["fp32"][pre + "geometry.10"].data_ptr()
+            for i, idx in enumerate((2, 4, 6, 8)):
+                a.w_geom_mid[i] = W[F][f"{pre}geometry.{idx}"].data_ptr()
+            a.w_combine = W[F][pre + "combine.0"].data_ptr()
+            a.w_combine_last = W["fp32"][pre + "combine.2"].data_ptr()
+        if "crop_in" in color:
+            a.crop_in = color["crop_in"].data_ptr()
+        else:
+            a.feats_t, a.pix = color["feats_t"].data_ptr(), color["pix"].data_ptr()
+            a.pairs, a.n_pairs = color["pairs"].data_ptr(), color["n_pairs"].data_ptr()
+            a.n_views, a.hw = int(color["n_views"]), int(color["hw"])
+        a.tables = self._ws("mask_tables", int(cplan.bytes), torch.uint8, dev).data_ptr()
+        a.canvas_bytes = 4 * 64 * (total * 4 if math == 0 else cvox * (2 if math == 2 else 4))
+        a.canvas = self._ws("mask_canvas", a.canvas_bytes, torch.uint8, dev).data_ptr()
+        if math == 2:
+            a.canvas32_bytes = cvox * (64 if only else 128) * 4
+            a.canvas32 = self._ws("mask_canvas32", a.canvas32_bytes, torch.uint8, dev).data_ptr()
+        outb = torch.empty(total * ncls, dtype=torch.float32, device=dev)
+        bits = torch.empty(total, dtype=torch.uint8, device=dev)
+        a.masks, a.bits, a.thresh = outb.data_ptr(), bits.data_ptr(), float(cfg.MASK_THRESH)
+        if extras is not None:
+            pin = self._ws("bits_host", total, torch.uint8, dev, pinned=True)
+            a.bits_host = pin.data_ptr()
+            extras.update(mask_bits=bits, mask_offsets=offs, mask_sizes=sizes, bits_pin=pin[:total])
+        tok = self._rec("mask_stage_color")
+        S.check(S.lib.sis3d_mask_stage_color_launch(C.byref(plan), C.byref(cplan), C.c_void_p(stage.data_ptr()), C.byref(a),
+                                                    S.stream()), "mask_stage_color")
+        self._rec_end(tok)
+        return _MaskList(outb, offs, sizes, ncls)
+
     # ------------------------------------------------------------------ forward
     _carve_layouts = {}
 
@@ -920,9 +1013,10 @@ class Network(nn.Module):
         dev = scene_t.device
         P = self._predictions
         scene = Act(scene_t, dims, 2, layout="ncdhw")
-        imageft = None
+        imageft = color_src = None
         if cfg.USE_IMAGES:
             imageft = self._backproject(blobs, killing_inds, dims, dev, fused)
+            color_src = self.__dict__.pop("_color_src", None)
             self._imageft_vc = imageft.t if (self._keep_debug and not isinstance(imageft, tuple)) else None
         level1, level2 = self._backbone(scene, imageft)
         if self._keep_debug:
@@ -932,6 +1026,10 @@ class Network(nn.Module):
         pack = torch.empty(total + 16, dtype=torch.uint8, device=dev)
         out, _ = self._carve(pack, R, nc)
         out["pack"] = pack
+        if color_src is not None:
+            # the colour-aware mask stage gathers its crops from these after the stage; referenced here, they outlive a
+            # captured graph's own use of them (its private pool would otherwise hand their memory to later layers)
+            out["color_src"] = color_src
         rois, scores, level_ids = out["rois"], out["scores"], out["level_ids"]
         num = out["num"][:1]
         out["num"] = num
@@ -1032,17 +1130,13 @@ class Network(nn.Module):
             gt = gt.cpu().numpy() if isinstance(gt, torch.Tensor) else np.asarray(gt)
             h.update(use_graph=False, fused=None, gt_box=gt,
                      gt_det=gt_detection_table(gt, dims, cfg.CLASS_THRESH, int(cfg.NUM_CLASSES)))
+            if self._mask_colour():  # its crops' image features come from the views (reference: network.py:194-239)
+                h["fused"] = self._fused_inputs(blobs, dims)
             return h
         with torch.no_grad(), Network._UseSlot(self, slot):
             lists = cfg.USE_IMAGES and "proj_ind_3d" in blobs
             use_graph = self._use_graph and not (self._keep_debug or self._prof is not None or lists)
-            fused = None
-            if cfg.USE_IMAGES and not lists:
-                imgs = blobs["nearest_images"]
-                w, hh = int(cfg.DEPTH_SHAPE[0]), int(cfg.DEPTH_SHAPE[1])
-                vp = proj.view_params(cfg.INTRINSIC, (w, hh), cfg.PROJ_DEPTH_MIN, cfg.PROJ_DEPTH_MAX, dims, None,
-                                      imgs["poses"][0], imgs["world2grid"][0])
-                fused = dict(vp=vp, feats=imgs["images"][0], depths=torch.as_tensor(imgs["depths"][0]))
+            fused = self._fused_inputs(blobs, dims) if cfg.USE_IMAGES else None
             h.update(use_graph=use_graph, fused=fused)
             if use_graph:
                 nv = fused["feats"].shape[0] if fused else 0
@@ -1070,6 +1164,32 @@ class Network(nn.Module):
                     h["fdev"] = None
                 h["st"] = st
         return h
+
+    @staticmethod
+    def _fused_inputs(blobs, dims):
+        """Per-view constants (host) and inputs of the on-device projection; None for blobs with precomputed index lists."""
+        if "proj_ind_3d" in blobs:
+            return None
+        imgs = blobs["nearest_images"]
+        w, hh = int(cfg.DEPTH_SHAPE[0]), int(cfg.DEPTH_SHAPE[1])
+        vp = proj.view_params(cfg.INTRINSIC, (w, hh), cfg.PROJ_DEPTH_MIN, cfg.PROJ_DEPTH_MAX, dims, None,
+                              imgs["poses"][0], imgs["world2grid"][0])
+        return dict(vp=vp, feats=imgs["images"][0], depths=torch.as_tensor(imgs["depths"][0]))
+
+    @staticmethod
+    def _fused_to(fused, dev):
+        return dict(vp=fused["vp"].to(dev, non_blocking=True), feats=fused["feats"].to(dev, torch.float32, non_blocking=True),
+                    depths=fused["depths"].to(dev, torch.float32, non_blocking=True).contiguous())
+
+    def _color_sources(self, blobs, killing_inds, dims, dev, fused):
+        """Ground-truth RoIs with a colour-aware mask head: the view maps and channels-last view features its gather reads,
+        made without the static stage (ENet when the views are images, projection maps, pairs; no feature volume)."""
+        feats, pix, pairs, n_pairs = self._view_maps(blobs, killing_inds, dims, dev, self._fused_to(fused, dev) if fused else None)
+        feats = feats.contiguous()
+        n, Cn, hw = feats.shape[0], feats.shape[1], feats.shape[2] * feats.shape[3]
+        feats_t = torch.empty(n, hw, Cn, dtype=torch.float32, device=dev)
+        S.check(S.lib.sis3d_mask_color_feats_t(S.ptr(feats), n, Cn, hw, S.ptr(feats_t), S.stream()), "mask_color_feats_t")
+        return dict(feats_t=feats_t, pix=pix, pairs=pairs, n_pairs=n_pairs, n_views=n, hw=hw)
 
     def _run_static(self, h):
         """Step 1b (async): static stage (graph replay) on the staged inputs, packed results -> pinned host (async D2H)."""
@@ -1123,16 +1243,18 @@ class Network(nn.Module):
                     outs = ring[st["ring_pos"]]
                     st["ring_pos"] ^= 1
                 outs["pack"].copy_(st["outs"]["pack"], non_blocking=True)
+                if "color_src" in st["outs"]:
+                    outs["color_src"] = st["outs"]["color_src"]
                 scene_t = st["scene"].clone() if h["fresh"] else st["scene"]
-            elif "gt_det" in h:  # ground-truth RoIs: the scene's input copy is its only work before the mask stage
+            elif "gt_det" in h:  # ground-truth RoIs: the scene's input copy (and a colour head's view maps) before the mask stage
                 scene_t = data.to(dev, torch.float32, non_blocking=True).contiguous()
                 outs = None
+                if self._mask_colour():
+                    h["color_src"] = self._color_sources(blobs, killing_inds, dims, dev, fused)
             else:
                 scene_t = data.to(dev, torch.float32, non_blocking=True).contiguous()
                 if fused:
-                    fused = dict(vp=fused["vp"].to(dev, non_blocking=True),
-                                 feats=fused["feats"].to(dev, torch.float32, non_blocking=True),
-                                 depths=fused["depths"].to(dev, torch.float32, non_blocking=True).contiguous())
+                    fused = self._fused_to(fused, dev)
                 outs = self._static_stage(scene_t, dims, blobs, killing_inds, fused)
             h["outs"], h["scene_t"] = outs, scene_t
             # the one host round trip of a scene: decoded detections with the RoI count in row 0 / col 15 (12.8 KB)
@@ -1169,7 +1291,7 @@ class Network(nn.Module):
                 if cfg.USE_MASK:
                     det_host = det_all[:n].copy()
                     extras = {}
-                    P["mask_pred"] = [self._mask_branch(h["scene_t"], det_host, n, extras)]
+                    P["mask_pred"] = [self._mask_branch(h["scene_t"], det_host, n, extras, outs.get("color_src"))]
                     P["detections_host"] = det_host
                     if "bits_pin" in extras:  # thresholded predicted-class masks -> pinned host (queued by the mask stage)
                         h["bits_pin"] = extras.pop("bits_pin")
@@ -1194,7 +1316,7 @@ class Network(nn.Module):
         with torch.no_grad(), Network._UseSlot(self, h["slot"]):
             if cfg.USE_MASK:
                 extras = {}
-                P["mask_pred"] = [self._mask_branch(h["scene_t"], det, n, extras)]
+                P["mask_pred"] = [self._mask_branch(h["scene_t"], det, n, extras, h.get("color_src"))]
                 if "bits_pin" in extras:
                     h["bits_pin"] = extras.pop("bits_pin")
                 P.update(extras)

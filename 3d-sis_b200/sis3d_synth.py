@@ -131,11 +131,13 @@ def _bottleneck(prefix, inpl, planes):
 
 
 def param_shapes(net="ScanNet_Backbone", use_images=True, num_classes=19, a1=3, a2=11,
-                 pool=4, rpn_channels=256, use_mask=True, only_images=False):
+                 pool=4, rpn_channels=256, use_mask=True, only_images=False, mask_images=None):
     """state_dict names -> shapes of the 3D part of the model (ENet excluded).
 
     ScanNet: lib/nets/backbones.py:171-231 (only_images: ONLY_IMAGES = USE_IMAGES = True, no geometry1 and a 128-channel
-    colour stack); SUNCG: 118-169; heads lib/nets/network.py:35-57; mask head lib/nets/backbones.py:236-253.
+    colour stack); SUNCG: 118-169; heads lib/nets/network.py:35-57; mask head lib/nets/backbones.py:236-272 (mask_images:
+    None, 'use' = MASK_USE_IMAGES: geometry ends 64 -> 64, a colour stack and combine; 'only' = MASK_ONLY_IMAGES too: the
+    colour stack's 1x1 makes the classes).
     """
     s = []
     if only_images:
@@ -185,14 +187,23 @@ def param_shapes(net="ScanNet_Backbone", use_images=True, num_classes=19, a1=3, 
         for i in (0, 2, 4, 6, 8):
             s += [(f"mask_backbone.geometry.{i}.weight", (64, cin, 3, 3, 3))]
             cin = 64
-        s += [("mask_backbone.geometry.10.weight", (num_classes, 64, 1, 1, 1))]
+        s += [("mask_backbone.geometry.10.weight", (64 if mask_images else num_classes, 64, 1, 1, 1))]
+        if mask_images:
+            cin = 128
+            for i in (0, 2, 4, 6, 8):
+                s += [(f"mask_backbone.color.{i}.weight", (64, cin, 3, 3, 3))]
+                cin = 64
+            s += [("mask_backbone.color.10.weight", (num_classes if mask_images == "only" else 64, 64, 1, 1, 1)),
+                  ("mask_backbone.combine.0.weight", (128, 128, 3, 3, 3)),
+                  ("mask_backbone.combine.2.weight", (num_classes, 128, 1, 1, 1))]
     return OrderedDict(s)
 
 
 # gains applied on top of the U(-1/sqrt(fan_in), 1/sqrt(fan_in)) default-init bound so that a
 # random network yields a non-degenerate workload (varied RPN scores, confident classes -> masks).
 _GAINS = {"rpn_cls_score_net": 40.0, "rpn_bbox_pred_net": 4.0, "classifier_cls_score_net": 60.0,
-          "classifier_bbox_pred_net": 3.0, "mask_backbone.geometry.10": 8.0}
+          "classifier_bbox_pred_net": 3.0, "mask_backbone.geometry.10": 8.0, "mask_backbone.color.10": 8.0,
+          "mask_backbone.combine.2": 8.0}
 
 
 def make_weights(seed=0, **kw):
@@ -257,13 +268,14 @@ def build_case(port, c):
     return cfg, w, data, views
 
 
-def make_net(c, keep_debug=True, math="fp32", weights=None, enet=False, gt_rois=None, only_images=False):
+def make_net(c, keep_debug=True, math="fp32", weights=None, enet=False, gt_rois=None, only_images=False, mask_images=None):
     """The product Network for a case: released yml config, seeded synthetic weights loaded through load_state_dict.
     enet=True: cfg.USE_IMAGES_GT=False -- the blobs carry RGB frames and the 2-D ENet encoder (seeded default init) is part
     of the forward.  gt_rois=True / False: test mode on ground-truth boxes and classes (USE_RPN = USE_CLASS = False) with
     USE_BACKBONE on / off; the weights are those of the same model without RPN and classifier heads (the ones
     oracle/make_golden_gt_rois.py loads into the reference).  only_images=True: the image-only ScanNet backbone (ONLY_IMAGES)
-    with the weights of param_shapes(only_images=True)."""
+    with the weights of param_shapes(only_images=True).  mask_images='use' / 'only': the colour-aware mask head
+    (MASK_USE_IMAGES, with MASK_ONLY_IMAGES for 'only') and the weights of param_shapes(mask_images=...)."""
     import os
     import torch
     from lib.utils.config import cfg, cfg_from_file, cfg_reset
@@ -273,6 +285,7 @@ def make_net(c, keep_debug=True, math="fp32", weights=None, enet=False, gt_rois=
     cfg.NUM_CLASSES = 26 if c["cfgname"] == "suncg" else 19
     cfg.USE_IMAGES, cfg.USE_MASK, cfg.USE_IMAGES_GT = c["use_images"], c["use_mask"], not enet
     cfg.ONLY_IMAGES = bool(only_images)
+    cfg.MASK_USE_IMAGES, cfg.MASK_ONLY_IMAGES = bool(mask_images), mask_images == "only"
     if gt_rois is not None:
         cfg.USE_RPN, cfg.USE_CLASS, cfg.USE_BACKBONE = False, False, bool(gt_rois)
     from lib.nets import backbones
@@ -282,11 +295,11 @@ def make_net(c, keep_debug=True, math="fp32", weights=None, enet=False, gt_rois=
     net.init_modules()
     if weights is None and gt_rois is not None:
         weights = {k: v for k, v in make_weights(seed=0, net=cfg.NET, use_images=c["use_images"], num_classes=cfg.NUM_CLASSES,
-                                                 a1=0, a2=0, use_mask=c["use_mask"]).items()
+                                                 a1=0, a2=0, use_mask=c["use_mask"], mask_images=mask_images).items()
                    if not k.startswith("classifier_")}
     w = weights if weights is not None else make_weights(
         seed=0, net=cfg.NET, use_images=c["use_images"], num_classes=cfg.NUM_CLASSES, a1=cfg.NUM_ANCHORS_LEVEL1,
-        a2=cfg.NUM_ANCHORS_LEVEL2, use_mask=c["use_mask"], only_images=only_images)
+        a2=cfg.NUM_ANCHORS_LEVEL2, use_mask=c["use_mask"], only_images=only_images, mask_images=mask_images)
     net.load_state_dict({k: torch.from_numpy(v) for k, v in w.items()}, strict=not enet)
     net._keep_debug = keep_debug
     net.set_conv_math(math)

@@ -364,6 +364,69 @@ typedef struct sis3d_mask_stage {
     int32_t reserved2;
 } sis3d_mask_stage;
 int sis3d_mask_stage_launch(const sis3d_mask_plan *plan, const void *h_blob, const sis3d_mask_stage *args, void *stream);
+
+/* Colour-aware mask head (MASK_USE_IMAGES / MASK_ONLY_IMAGES; lib/nets/backbones.py:236-287, lib/nets/network.py:302-317):
+ * mask = sigmoid(combine(cat[geometry(scene crop), color(imageft crop)])), or sigmoid(color(imageft crop)) with only_images.
+ * imageft is the 128-channel back-projected volume (max over the paired views, 0 where a view sees nothing); it is never
+ * built: every kept crop's channels are gathered onto the stage input from the per-view maps (csrc/mask_color.cu).
+ *
+ * sis3d_mask_color_plan_build appends the colour stage's tables to a blob that sis3d_mask_plan_build has just filled for the
+ * same h_det (plan = its result; canvas mode when plan->n_tiles_tc > 0): crops int32[n_kept][8] = x0, y0, z0, w, h, l, canvas
+ * x, 0; region tables of the 1x1 convs that write a half of the 128-channel concatenation (g2c), of combine's 1x1 (last128),
+ * and, on compact buffers only, of colour.0 (128 -> 64) and combine.0 (128 -> 128).  cplan->bytes = the blob's whole size
+ * (ship it with one H2D copy); SIS3D_EWORKSPACE when capacity is smaller. */
+typedef struct sis3d_mask_color_plan {
+    int64_t off_crops, off_g2c, off_last128, off_c0, off_c128, bytes;
+} sis3d_mask_color_plan;
+int sis3d_mask_color_plan_build(const float *h_det, int n, const sis3d_mask_plan *plan, void *h_blob, size_t capacity,
+                                sis3d_mask_color_plan *cplan);
+/* The gather: for every voxel of every crop, out[row][c] = max over the (feature map, index map) pairs of
+ * (pix[map][voxel] >= 0 ? feats_t[feat][pix][c] : 0), the first pair's value taken as it is -- sis3d_backproject_max's value
+ * at that voxel, bit for bit.  feats_t [n_views][hw][C] channels-last features, pix int16[n_views][Z*Y*X], pairs / n_pairs
+ * from sis3d_backproject_pairs (or the caller's pairing); crops / offs as in the plans above.  layout 0: compact fp32
+ * rows (row = offs[j] + voxel); 1: fp32 canvas [.][cy][cz][C] at x = crops[j][6] + x; 2: the same canvas in fp16 (round to
+ * nearest).  Voxels outside the crops are not written.  C % 4 == 0. */
+int sis3d_mask_color_gather(const float *feats_t, const int16_t *pix, const int32_t *pairs, const int32_t *n_pairs, int n_views,
+                            int C, int hw, int X, int Y, int Z, const int32_t *crops, const int64_t *offs, int n_crops,
+                            int64_t total, int cy, int cz, int layout, void *out, void *stream);
+/* [n_views][C][hw] -> [n_views][hw][C] (the gather's feats_t when no back-projection made one) */
+int sis3d_mask_color_feats_t(const float *feats, int n_views, int C, int hw, float *feats_t, void *stream);
+/* Every launch of a colour-aware scene's mask stage behind one call, on the routes of sis3d_mask_stage_launch (math 0 compact
+ * fp32 CUDA-core, 1 TF32 canvas, 2 fp16-operand canvas).  Layers: colour input (gather, or crop_in: a dense fp32 VC crop
+ * [w][h][l][128] of the single kept RoI, copied), color.0 .. color.8, color.10 -> channels [64, 128) of the concatenation
+ * (only_images: -> sigmoid masks), geometry.0 .. geometry.8, geometry.10 -> channels [0, 64), combine.0, combine.2 ->
+ * sigmoid masks, the predicted-class select, bits and their D2H.  Weights: *_first / *_last / *_combine_last fp32
+ * (sis3d_pack_conv_weight); *_mid and w_color_first / w_combine packed for `math` as w_mid of sis3d_mask_stage.  geometry
+ * and combine weights are not read with only_images.  canvas_bytes >= 4 x voxels (compact total or canvas) x 64 channels in
+ * the operand type; math 2: canvas32_bytes >= canvas voxels x 128 (only_images: 64) x 4. */
+typedef struct sis3d_mask_stage_color {
+    const float *scene;            /* NCDHW [2][X][Y][Z] */
+    int32_t X, Y, Z, ncls, math, only_images;
+    const float *w_geom_first, *w_geom_last;
+    const void *w_geom_mid[4];
+    const void *w_color_first;
+    const void *w_color_mid[4];
+    const float *w_color_last;
+    const void *w_combine;
+    const float *w_combine_last;
+    const float *feats_t;          /* gather inputs (see sis3d_mask_color_gather) */
+    const int16_t *pix;
+    const int32_t *pairs, *n_pairs;
+    int32_t n_views, hw;
+    const float *crop_in;          /* instead of the gather (n_kept must be 1), or NULL */
+    void *tables;                  /* device, >= cplan->bytes */
+    void *canvas;
+    size_t canvas_bytes;
+    float *canvas32;
+    size_t canvas32_bytes;
+    float *masks;
+    uint8_t *bits;
+    uint8_t *bits_host;
+    float thresh;
+    int32_t reserved;
+} sis3d_mask_stage_color;
+int sis3d_mask_stage_color_launch(const sis3d_mask_plan *plan, const sis3d_mask_color_plan *cplan, const void *h_blob,
+                                  const sis3d_mask_stage_color *args, void *stream);
 /* cudaMemcpyAsync behind the C ABI (kind 1 H2D, 2 D2H, 3 D2D) for hosts that stage their own pinned buffers. */
 int sis3d_memcpy_async(void *dst, const void *src, size_t bytes, int kind, void *stream);
 
